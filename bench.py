@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- BASELINE.json's metric on B200s: SAE training tokens/sec + run_with_cache images/sec, % of roofline.
+"""bench.py -- BASELINE.json's metric on H100s: SAE training tokens/sec + run_with_cache images/sec, % of roofline.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload all|sae|vit]
                     [--dtype fp32|bf16] [--batch B] [--model b32|l14]
@@ -18,7 +18,7 @@ Per record:
              step's result inside the timed region
   roofline   SAE: the step's algorithmic bytes (SURVEY 8d: 80 d F + 8 Bt d) / step time against the measured HBM copy
              bandwidth, plus live CUDA-event timings of every stage; ViT: the dominant GEMM's algorithmic flops against the
-             measured bf16 peak.  ``traffic`` is read from the committed ncu summary under profiles/ (null if none matches).
+             measured bf16 peak.  ``traffic`` is read from an ncu summary under profiles/ when one is present (null otherwise).
   cpu_baseline  the oracle port (oracle/*.py) timed on this box's host cores on a bounded sample
   dp_parity  (N > 1) after the timed region every rank re-trains the reference-made fixture tests/golden/sae_tiny_b.pt through
              ``VisionSAETrainer(p2p_group=...)`` and compares losses, TopK indices, parameters and counters with the
@@ -46,6 +46,47 @@ import torch  # noqa: E402
 SAE_CFG = dict(d_in=768, expansion=32, k=32, batch=4096, dtype="float32")     # BASELINE.json configs[2]
 SAE_CFG5 = dict(d_in=768, expansion=128, k=32, batch=4096, dtype="bfloat16")  # BASELINE.json configs[4]: dict 768x128, bf16, data parallel
 POOL_BATCHES = 16                                            # synthetic activation pool = 16 steps' worth of tokens (201 MB > L2)
+DUMP_BUDGET_BYTES = 64 << 20                                 # --dump-outputs: all files together
+DUMP_MAX_ELEMS = 1 << 21                                     # per array; a larger output is written as a fixed, seeded sample
+DUMP_HOOK_ELEMS = 1 << 14                                    # per hook point of a run_with_cache record (214 of them at ViT-B/32)
+
+
+class OutputDump:
+    """--dump-outputs DIR: what a timed path computed in its last timed step, one ``DIR/<name>.npy`` per array (float32; float64
+    for integer outputs so indices stay exact).  An array of more than ``max_elems`` elements is written as the elements at a
+    sorted random draw of flat positions from a generator seeded with the array's size, so two builds given the same
+    arguments write the same positions and can be compared output for output."""
+
+    def __init__(self, path):
+        self.path, self.total = path, 0
+        if path:
+            os.makedirs(path, exist_ok=True)
+
+    def __bool__(self):
+        return bool(self.path)
+
+    def add(self, name, t, max_elems=DUMP_MAX_ELEMS):
+        import numpy as np
+        if not self.path or t is None:
+            return
+        t = torch.as_tensor(t).detach().reshape(-1)
+        if t.numel() > max_elems:
+            g = torch.Generator().manual_seed(t.numel())
+            pos = torch.randint(0, t.numel(), (max_elems,), generator=g).sort().values
+            t = t[pos.to(t.device)]
+        exact = t.dtype in (torch.float64, torch.int64, torch.int32, torch.int16, torch.int8, torch.uint8, torch.bool)
+        a = t.to("cpu", torch.float64 if exact else torch.float32).numpy()
+        self.total += a.nbytes
+        if self.total > DUMP_BUDGET_BYTES:
+            raise SystemExit(f"bench.py: --dump-outputs would exceed {DUMP_BUDGET_BYTES >> 20} MB at {name}")
+        np.save(os.path.join(self.path, name + ".npy"), a)
+
+    def train_step(self, tag, out, sae):
+        """VisionSAETrainer.train_step's results and the parameters it updated in place."""
+        for name, v in zip(("loss", "mse_loss", "l1_loss", "l0", "act_freq_scores", "n_forward_passes_since_fired", "n_frac_active_tokens"), out):
+            self.add(f"{tag}.{name}", v)
+        for name in ("W_enc", "W_dec", "b_enc", "b_dec"):
+            self.add(f"{tag}.{name}", getattr(sae, name))
 
 
 def _peaks():
@@ -55,7 +96,8 @@ def _peaks():
         return {"hbm_gbs": p["hbm_gbs"], "bf16_tflops": p["bf16_tflops"], "bf16_tflops_sustained": p.get("bf16_tflops_sustained"),
                 "source": "measured"}
     except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
+        # H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense bf16 -- a ceiling, not a measured rate
+        return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": None, "source": "H100 SXM data sheet"}
 
 
 def ncu_traffic(kernel_regex: str, prefer: str = ""):
@@ -86,7 +128,7 @@ def ncu_traffic(kernel_regex: str, prefer: str = ""):
 
 
 class ClockSampler:
-    """SM clock / throttle reasons sampled DURING the timed region (B200_PROFILING.md), through NVML in this process.
+    """SM clock / throttle reasons sampled DURING the timed region, through NVML in this process.
 
     NVML is initialised when the sampler is constructed (before the warm-up steps): starting `nvidia-smi` next to the timed
     loop costs seconds of driver initialisation that stall this process's own launches, and its first sample arrives after a
@@ -358,7 +400,7 @@ def time_dominant_gemm(model, batch, dtype, iters=10):
     return {"ms": ms, "flops": 2.0 * M * N * K, "bytes": float(M * K * es + N * K * es + 2 * M * N * es), "shape": [M, N, K]}
 
 
-def run_vit(args, ctx, cpu_leg=True):
+def run_vit(args, ctx, cpu_leg=True, dump=None):
     from vit_prisma.b200 import _lib as L
     from vit_prisma.b200.synthetic import CLIP_B32, CLIP_L14
     world, rank, dev = ctx.world, ctx.rank, ctx.dev
@@ -385,14 +427,21 @@ def run_vit(args, ctx, cpu_leg=True):
     with clocks:
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
-        for _ in range(args.steps):
+        for i in range(args.steps):
             out, cache = model.run_with_cache(x, **run_kw)
             n_keys = len(cache)
-            del cache
+            if i < args.steps - 1 or not (dump and rank == 0):
+                del cache
         e1.record()
         ctx.barrier()
         dev_ms = ctx.max_over_ranks(e0.elapsed_time(e1))
     clocks.close()
+    if dump and rank == 0:
+        tag = "vit_" + args.dtype
+        dump.add(f"{tag}.out", out)
+        for name, act in cache.items():
+            dump.add(f"{tag}.cache.{name}", act, DUMP_HOOK_ELEMS)
+        del cache
     launches = L.get_lib().pb_launch_count() - launches0
     route = model.last_route
 
@@ -435,19 +484,19 @@ def run_vit(args, ctx, cpu_leg=True):
     fp32 = dtype == torch.float32
     # fp32 mode executes 3 tensor-core passes per algorithmic flop; the roofline counts ALGORITHMIC flops
     achieved = kern["flops"] / (kern["ms"] / 1e3) / 1e12
-    traffic, traffic_src = (None, None) if l14 else ncu_traffic(r"k_gemm_tc2<float" if fp32 else r"k_gemm_tc2<__nv_bfloat16|k_gemm_tc2<bf16",
+    traffic, traffic_src = (None, None) if l14 else ncu_traffic(r"k_gemm_tc<float" if fp32 else r"k_gemm_tc<__nv_bfloat16|k_gemm_tc<bf16",
                                                                 prefer="gemm_fp32" if fp32 else "gemm_bf16")
-    # the tensor core runs kind::tf32 at half the kind::f16 rate: the fp32-mode denominator is bf16_peak / 2 per executed pass,
+    # the tensor core runs tf32 wgmma at half the bf16 rate: the fp32-mode denominator is bf16_peak / 2 per executed pass,
     # i.e. bf16_peak / 6 per algorithmic flop of the 3-pass product (MEASURED_PEAKS.json has no TF32 entry; derived, not measured)
     mode_peak = peaks["bf16_tflops"] / 6 if fp32 else peaks["bf16_tflops"]
-    roof = {"bound": "tensor", "kernel": "k_gemm_tc2 (MLP-in GEMM + bias + GELU, hook_pre/hook_post spill)", "achieved": achieved,
+    roof = {"bound": "tensor", "kernel": "k_gemm_tc (MLP-in GEMM + bias + GELU, hook_pre/hook_post spill)", "achieved": achieved,
             "peak": peaks["bf16_tflops"], "unit": "TFLOP/s", "frac": achieved / peaks["bf16_tflops"], "traffic": traffic,
             "traffic_source": traffic_src, "traffic_unit": "B/launch (ncu dram read+write)", "algorithmic_bytes": kern["bytes"],
             "executed_tensor_tflops": achieved * (3 if fp32 else 1),
             "mode_peak": mode_peak, "mode_frac": achieved / mode_peak,
-            "mode_peak_source": ("bf16_tflops / 2 (kind::tf32 runs at half the kind::f16 rate) / 3 passes -- derived from the measured bf16 peak"
-                                 if fp32 else "measured bf16 burst"),
-            "peak_source": peaks["source"] + " bf16 burst (kernel timed alone)", "shape_MNK": kern["shape"], "kernel_ms": kern["ms"],
+            "mode_peak_source": (f"bf16 peak ({peaks['source']}) / 2 (tf32 wgmma runs at half the bf16 rate) / 3 passes"
+                                 if fp32 else f"bf16 peak ({peaks['source']})"),
+            "peak_source": peaks["source"] + " bf16 peak (kernel timed alone)", "shape_MNK": kern["shape"], "kernel_ms": kern["ms"],
             "hbm_gbs_of_kernel": kern["bytes"] / (kern["ms"] / 1e3) / 1e9, "hbm_peak_gbs": peaks["hbm_gbs"],
             "passes": 3 if fp32 else 1,
             "step_algorithmic_tflops": flops_img * imgs / (dev_ms / 1e3) / 1e12,
@@ -461,8 +510,8 @@ def run_vit(args, ctx, cpu_leg=True):
            "config": {"workload": f"vit_l14_run_with_cache_resid_post_l{args.layer}" if l14 else "vit_b32_run_with_cache_all_hooks",
                       "model": ("CLIP ViT-L/14" if l14 else "CLIP ViT-B/32") + " geometry, seeded synthetic weights",
                       "batch_per_gpu": B, "global_batch": B * world, "hook_points_cached": n_keys, "route": route,
-                      "gemm": "tcgen05 3xTF32" if fp32 else "tcgen05 bf16",
-                      "cache_bytes_per_image": int(cache_b_img * es / 4), "l2": "working set (activations of one layer >> 126 MB) larger than L2",
+                      "gemm": "wgmma 3xTF32" if fp32 else "wgmma bf16",
+                      "cache_bytes_per_image": int(cache_b_img * es / 4), "l2": "working set (activations of one layer >> 50 MB) larger than L2",
                       "parallelism": f"dp{world} (images sharded, no collective)"},
            "clocks": clocks.summary(), "gpu_launches": int(launches),
            "e2e": {"value": e2e, "unit": "images/s", "h2d_bytes_per_step": int(host.numel() * host.element_size()),
@@ -528,7 +577,7 @@ def build_sae_trainer(ctx, cfg, store, group=None, init=None):
     return trainer
 
 
-def run_sae(args, ctx, spec=None):
+def run_sae(args, ctx, spec=None, dump=None):
     """``spec`` = SAE_CFG (the headline, configs[2]) or SAE_CFG5 (configs[4]: bf16 storage -- parameters, state dict and activations
     in bf16; the step engine trains fp32 masters and exports the rounded parameters every step, vit_prisma/sae/sae.py)."""
     from vit_prisma.b200 import _lib as L
@@ -563,6 +612,7 @@ def run_sae(args, ctx, spec=None):
         state["step"] += 1
         state["tokens"] += Bt * world
         state["n_frac"] = out[-1]
+        state["out"] = out
         return out[0]                                     # loss: 0-dim device tensor
 
     clocks = ClockSampler(ctx.local, period_s=0.002)
@@ -583,6 +633,8 @@ def run_sae(args, ctx, spec=None):
     clocks.close()
     launches = L.get_lib().pb_launch_count() - l0
     assert sae.step_engine() is eng, "the step engine was rebuilt during training"
+    if dump and rank == 0:
+        dump.train_step("sae" if spec is SAE_CFG else "sae_cfg5", state["out"], sae)
 
     # ---- e2e: pinned host tokens -> H2D -> VisionSAETrainer.train_step -> D2H of the step's loss
     loss_host = torch.empty(1).pin_memory()
@@ -635,8 +687,8 @@ def run_sae(args, ctx, spec=None):
     traffic_total = sum(e["traffic"] for e in with_ncu) if with_ncu and all(e["traffic"] is not None for e in with_ncu) else None
     roof = {"bound": "hbm", "kernel": "whole training step (SURVEY 8d: 80 d F + 8 Bt d algorithmic bytes; weights + gradients + Adam state dominate)",
             "achieved": step_gbs, "peak": peaks["hbm_gbs"], "unit": "GB/s", "frac": step_gbs / peaks["hbm_gbs"],
-            "traffic": traffic_total, "traffic_unit": "B/step (sum of the stages' ncu dram read+write, committed summaries under profiles/)",
-            "algorithmic_bytes": step_bytes, "peak_source": peaks["source"] + " HBM copy bandwidth",
+            "traffic": traffic_total, "traffic_unit": "B/step (sum of the stages' ncu dram read+write, summaries under profiles/ when present)",
+            "algorithmic_bytes": step_bytes, "peak_source": peaks["source"] + (" HBM copy bandwidth" if peaks["source"] == "measured" else " HBM bandwidth"),
             "dominant_kernel": dom, "stages": kernels}
     cpu = cpu_sae_tokens_per_sec()
     mb = d * F * 4 / 1e6
@@ -664,7 +716,7 @@ def run_sae(args, ctx, spec=None):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-def run_sae_forward(args, ctx, expansion=64):
+def run_sae_forward(args, ctx, expansion=64, dump=None):
     """north_star's forward-only shape: SAE encoder -> TopK -> decoder at d_model 768, dict 768 x 64, 4096 tokens per call,
     against SURVEY 8(d)'s forward bytes `4*(2*Bt*d) + 4*d*F + 4*F + 4*d*min(F, Bt*k)` (sparse outputs; no dense feature_acts).
     Every rank runs its own replica (no collective); the record reports the sum."""
@@ -677,7 +729,7 @@ def run_sae_forward(args, ctx, expansion=64):
     unit_norm_rows_(eng.W_dec)
     eng.refresh_lo()
     pool = activation_pool(Bt * 8, d, seed=ctx.rank).to(ctx.dev)
-    n = max(args.steps, 10)
+    n = args.steps
     # warm-up by time, not by count: on rank 0 this record follows ~12 s of host-only work (the CPU baseline) during which the GPU
     # idles and drops its clocks; a handful of 0.7 ms calls is not enough to bring them back before the timed region starts
     t_warm, i = time.perf_counter(), 0
@@ -692,10 +744,13 @@ def run_sae_forward(args, ctx, expansion=64):
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for i in range(n):
-        eng.forward(pool[(i % 8) * Bt:(i % 8 + 1) * Bt])
+        res = eng.forward(pool[(i % 8) * Bt:(i % 8 + 1) * Bt])
     e1.record()
     ctx.barrier()
     ms = ctx.max_over_ranks(e0.elapsed_time(e1)) / n
+    if dump and ctx.rank == 0:
+        for name, v in zip(("sae_out", "idx", "val"), res):
+            dump.add(f"sae_fwd.{name}", v)
     fb_rows, rescored = eng.fallback_rows(), eng.rescored_per_row(Bt)
 
     def phase_ms(bits, reps=5):                       # one phase of the fused encode alone, warm replays
@@ -732,11 +787,11 @@ def run_sae_forward(args, ctx, expansion=64):
                          "note": "the candidate GEMM is one TF32 tensor-core pass (fp32-exact TopK indices against the reference need at "
                                  "least that): the call is tensor-bound, not HBM-bound",
                          "encoder_tf32_frac": 2.0 * Bt * F * d / (ms / 1e3) / 1e12 / tf32_peak,
-                         "tf32_peak_tflops": tf32_peak, "tf32_peak_source": "bf16 burst peak of MEASURED_PEAKS.json / 2"}}
+                         "tf32_peak_tflops": tf32_peak, "tf32_peak_source": f"bf16 peak ({peaks['source']}) / 2"}}
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-def run_cfg4(args, ctx):
+def run_cfg4(args, ctx, dump=None):
     """BASELINE.json configs[3]: CLIP ViT-L/14 run_with_cache feeding an SAE (d_model 1024, dict 1024 x 64, TopK 32), data parallel:
     every rank runs its own VisionActivationsStore over its own synthetic image shard (names_filter = one resid_post,
     stop_at_layer = layer + 1, exactly the store's call) and trains on its own token shard through VisionSAETrainer.train_step;
@@ -776,6 +831,7 @@ def run_cfg4(args, ctx):
                                  n_training_steps=state["step"], n_training_tokens=state["step"] * Bt * world)
         state["step"] += 1
         state["n_frac"] = out[-1]
+        state["out"] = out
         return out[0]
 
     for _ in range(args.warmup):
@@ -788,6 +844,8 @@ def run_cfg4(args, ctx):
     e1.record()
     ctx.barrier()
     ms = ctx.max_over_ranks(e0.elapsed_time(e1))
+    if dump and rank == 0:
+        dump.train_step("cfg4", state["out"], sae)
     if rank != 0:
         return None
     tokens = world * Bt * args.steps
@@ -896,31 +954,36 @@ def main():
     ap.add_argument("--batch", type=int, default=512, help="ViT images per step per GPU")
     ap.add_argument("--model", default="b32", choices=["b32", "l14"], help="l14 = cfg #4: ViT-L/14 with the activation store's names_filter / stop_at_layer")
     ap.add_argument("--layer", type=int, default=22, help="hook_resid_post layer cached by --model l14")
-    ap.add_argument("--vit-steps", type=int, default=None, help="steps of the secondary ViT record under --workload all (default: min(steps, 10))")
+    ap.add_argument("--vit-steps", type=int, default=None, help="steps of the secondary ViT records under --workload all (default: --steps)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps write what each timed path computed in its last step as DIR/<name>.npy (float32 / float64)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.impl == "reference":
         return run_reference_arm(args)
     if not torch.cuda.is_available():
         raise SystemExit("bench.py: no CUDA device -- the product path has no CPU fallback (use --impl reference for the CPU arm)")
     ctx = Ctx()
+    dump = OutputDump(args.dump_outputs if ctx.rank == 0 else None)
     rc = 0
     try:
         line = None
         if args.workload == "cfg4":
-            line = run_cfg4(args, ctx)
+            line = run_cfg4(args, ctx, dump=dump)
         if args.workload == "cfg5":
-            line = run_sae(args, ctx, spec=SAE_CFG5)
+            line = run_sae(args, ctx, spec=SAE_CFG5, dump=dump)
         if args.workload == "sae_fwd":
-            line = run_sae_forward(args, ctx)
+            line = run_sae_forward(args, ctx, dump=dump)
         if args.workload in ("all", "sae"):
-            line = run_sae(args, ctx)
+            line = run_sae(args, ctx, dump=dump)
             if ctx.world > 1:
                 ok, detail = dp_parity_gate(ctx)
                 if line is not None:
                     line["dp_parity"], line["dp_parity_detail"] = ok, detail
                 rc = 0 if ok else 3
             try:                                           # north_star's forward-only shape (dict 768 x 64), nested; never costs the headline
-                fwd = run_sae_forward(args, ctx)
+                fwd = run_sae_forward(args, ctx, dump=dump)
             except Exception as e:                         # noqa: BLE001 -- reported in the line, not swallowed
                 fwd = {"error": f"{type(e).__name__}: {e}"}
             if line is not None and fwd is not None:
@@ -928,16 +991,16 @@ def main():
         if args.workload in ("all", "vit"):
             vargs = argparse.Namespace(**vars(args))
             if args.workload == "all":
-                vargs.steps = args.vit_steps or min(args.steps, 10)
+                vargs.steps = args.vit_steps or args.steps
                 vargs.warmup = min(args.warmup, 3)
-            vit = run_vit(vargs, ctx)
+            vit = run_vit(vargs, ctx, dump=dump)
             if args.workload == "vit":
                 line = vit
             elif line is not None:
                 line["secondary"] = vit
             if args.workload == "all" and args.dtype == "fp32":      # the throughput mode of the same path: bf16 operands, fp32 accumulation
                 vargs.dtype = "bf16"
-                vit16 = run_vit(vargs, ctx, cpu_leg=False)
+                vit16 = run_vit(vargs, ctx, cpu_leg=False, dump=dump)
                 if line is not None and vit16 is not None:
                     vit16["cpu_baseline"] = vit["cpu_baseline"] if vit else None
                     line["secondary_bf16"] = vit16

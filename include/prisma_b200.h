@@ -1,5 +1,5 @@
 /*
- * prisma_b200.h -- C ABI of libprisma_b200.so (sm_100a).
+ * prisma_b200.h -- C ABI of libprisma_b200.so (sm_90a).
  *
  * The reference (Prisma-Multimodal/ViT-Prisma) has no FFI: its two hot paths are Python
  * methods that hand every flop to PyTorch ATen.  This header is the boundary a maintainer
@@ -60,9 +60,9 @@ PB_API int pb_abi_sizeof(int which);
  * With n_split > 1 the N axis is cut into n_split blocks of split_n columns and block j
  * of out0 goes to out_split[j] (row stride ld0): one launch fills hook_q / hook_k / hook_v.
  * dtype PB_F32 : impl SIMT  -> exact fp32 FFMA;
- *                impl TC    -> tcgen05 kind::tf32 in 3 passes (A, A_lo, B, B_lo all required;
+ *                impl TC    -> tf32 wgmma in 3 passes (A, A_lo, B, B_lo all required;
  *                              *_lo = x - tf32_trunc(x), see pb_split_tf32) ~fp32 accuracy.
- * dtype PB_BF16: impl TC    -> tcgen05 kind::f16 (bf16 in, fp32 accumulate in TMEM).
+ * dtype PB_BF16: impl TC    -> bf16 wgmma (bf16 in, fp32 accumulate in registers).
  * impl AUTO picks TC when the shape/alignment allows it, else SIMT.                         */
 typedef struct {
   int32_t M, N, K;
@@ -268,7 +268,7 @@ PB_API int pb_unit_norm_rows(float* W, float* W_lo, int32_t F, int32_t d, pb_str
 
 /* ------------------------------------------------ fused encoder -> TopK (no dense hidden_pre in HBM)
  * Replaces `hidden_pre = sae_in @ W_enc + b_enc` (sae/sae.py:568-574) + `torch.topk(hidden_pre, k)` (TopK.forward, :803-805) by
- *   phase 1  one-pass TF32 tcgen05 GEMM whose epilogue keeps, per token and per 128-feature segment, the c_keep largest
+ *   phase 1  one-pass TF32 wgmma GEMM whose epilogue keeps, per token and per 128-feature segment, the c_keep largest
  *            values as packed keys (cand: int32 [rows][d_sae / 128][c_keep]);
  *   phase 2  per token: the m_cand best keys (16 more per round, up to 128, while the proof below fails), EXACT fp32
  *            re-evaluation of those pre-activations, exact top-k of them, and a completeness proof with the per-row bound

@@ -12,12 +12,14 @@ What the CUDA path does instead, and what is modelled here step by step:
      value; bound on everything not re-scored:
          u = max( best key not re-scored ,  last kept key of every segment whose C kept keys were all re-scored )
          ub = upper end of u's value bucket (low 7 bits set)
-         E  = coef * (||a - trunc(a)|| max_f ||w_f|| + ||a|| max_f ||w_f - trunc(w_f)||) + 2^-13 |tau_k|
+         E  = coef * (||a - trunc(a)|| max_f ||w_f|| + ||a|| max_f ||w_f - trunc(w_f)||)
+              + ceil(d / 8) 2^-21 ||a|| max_f ||w_f|| + 2^-13 |tau_k|
      the row is PROVEN when ub + E < tau_k; otherwise 16 more candidates are re-scored (up to 128), then the row goes to the exact path;
   3. exact path (k_topk_fallback): top-k of the exact values of the whole row.
 
-The model computes the tf32 product with exact (float64) accumulation: the tensor core's accumulation error is what the safety factor
-``coef`` (1.05) and the 2^-13 |tau_k| term are there for.  Only tests/ may import this file.
+The model computes the tf32 product with exact (float64) accumulation: the tensor core's fp32 accumulation over ceil(d / 8) k-steps is
+what the ceil(d / 8) 2^-21 ||a|| max ||w|| term bounds (4 units of 2^-23 per step against magnitudes <= ||a|| max ||w||); ``coef``
+(1.05) covers the norms being evaluated in fp32, and the 2^-13 |tau_k| term the rounding of the bias add and of the key bucket.  Only tests/ may import this file.
 """
 from __future__ import annotations
 
@@ -27,7 +29,7 @@ SEG = 128
 
 
 def tf32_trunc(x: np.ndarray) -> np.ndarray:
-    """What a kind::tf32 tensor-core read sees of an fp32 value: the low 13 mantissa bits are ignored."""
+    """What a tf32 wgmma tensor-core read sees of an fp32 value: the low 13 mantissa bits are ignored."""
     return (np.asarray(x, dtype=np.float32).view(np.uint32) & np.uint32(0xFFFFE000)).view(np.float32)
 
 
@@ -93,7 +95,7 @@ def select_row(a: np.ndarray, W: np.ndarray, b: np.ndarray, k: int, c_keep: int 
         if sat.size:
             u = sat.max() if u is None else max(u, sat.max())
         u_val = -np.inf if u is None else float(ord2f(np.int32((int(u) & ~127) | 127)))
-        E = coef * (a_lo * w_norm + a_norm * w_lo) + abs(tau_k) * 2.0 ** -13
+        E = coef * (a_lo * w_norm + a_norm * w_lo) + -(-a.shape[0] // 8) * 2.0 ** -21 * a_norm * w_norm + abs(tau_k) * 2.0 ** -13
         proven = m_cur >= k and (u_val + E < tau_k)
         if proven or m_cur >= Gs:
             break

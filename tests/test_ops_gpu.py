@@ -66,8 +66,8 @@ def test_gemm_tc_bf16_matches_simt(M, N, K):
     pre_t, post_t = ops.gemm(a, w, b, act="gelu", want_post=True, impl=L.GEMM_TC)
     torch.cuda.synchronize()
     ref = a.float().cpu() @ w.float().cpu().t() + b.float().cpu()
-    assert rel_err(pre_t.float(), ref) < 1e-2, "tcgen05 bf16 vs fp32 reference"
-    assert rel_err(pre_t.float(), pre_s.float()) < 8e-3, "tcgen05 bf16 vs FFMA on the same bf16 inputs"
+    assert rel_err(pre_t.float(), ref) < 1e-2, "wgmma bf16 vs fp32 reference"
+    assert rel_err(pre_t.float(), pre_s.float()) < 8e-3, "wgmma bf16 vs FFMA on the same bf16 inputs"
     assert rel_err(post_t.float(), post_s.float()) < 8e-3
 
 
@@ -85,7 +85,7 @@ def test_gemm_tc_3xtf32_matches_fp32(M, N, K):
 
 
 def test_gemm_tc_3xtf32_m_fast_raster():
-    """Dictionary-sized B (> 48 MB with its lo plane) flips the persistent kernel to the m-fastest tile walk (SAE encoder shape)."""
+    """Dictionary-sized B (> 24 MB with its lo plane) flips the persistent kernel to the m-fastest tile walk (SAE encoder shape)."""
     ops, L = _ops(), _L()
     M, N, K = 520, 24576, 768
     a, w, b = _rand(M, K, seed=1).cuda(), _rand(N, K, seed=2, scale=K ** -0.5).cuda(), _rand(N, seed=3).cuda()

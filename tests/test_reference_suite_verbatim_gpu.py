@@ -1,4 +1,4 @@
-"""The reference's four offline test files run UNCHANGED against this package on a B200 (VERDICT r1 item 7e, SURVEY #26).
+"""The reference's four offline test files run UNCHANGED against this package on an H100 (VERDICT r1 item 7e, SURVEY #26).
 
 The files under tests/golden/ref_tests/ are verbatim copies (see the README there).  They import ``vit_prisma`` -- here that resolves to
 vit-prisma_b200/vit_prisma -- build host-resident models and feed host tensors; the package stages them on the GPU."""

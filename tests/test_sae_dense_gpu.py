@@ -1,6 +1,6 @@
 """Dense ReLU + L1 training step and ghost grads (csrc/sae_dense.cu, vit_prisma/b200/sae_dense.py) against the reference
 fixtures (tests/golden/sae_tiny_{d,e,f}.pt: torch autograd + torch.optim.Adam on the unmodified reference module) and, at a
-size that reaches the tcgen05 GEMMs, against the pinned oracle."""
+size that reaches the wgmma GEMMs, against the pinned oracle."""
 import math
 
 import pytest
@@ -36,7 +36,7 @@ def test_glue_kernels_match_torch():
     x = torch.randn(77, 133, generator=g).cuda()
     xt, lo = D.transpose(x)
     assert torch.equal(xt, x.t().contiguous())
-    hi = (xt.view(torch.int32) & -8192).view(torch.float32)                 # what kind::tf32 reads of the value
+    hi = (xt.view(torch.int32) & -8192).view(torch.float32)                 # what a tf32 wgmma reads of the value
     # lo plane = (x - hi) rounded to the nearest tf32: low 13 mantissa bits clear, within half a tf32 ulp of the exact remainder
     assert int((lo.view(torch.int32) & 8191).abs().max()) == 0
     assert float((lo - (xt - hi)).abs().max()) <= float((xt - hi).abs().max()) * 2.0 ** -11
@@ -98,7 +98,7 @@ def test_dense_and_ghost_steps_match_reference_golden(tag):
 
 @pytest.mark.parametrize("ghost,impl", [(False, "tc"), (True, "simt"), (True, "tc")])
 def test_dense_step_midsize_matches_oracle(ghost, impl):
-    """d=256, F=2048, 512 tokens: every product takes the tcgen05 3xTF32 GEMM ("tc") or the exact-fp32 FFMA kernel ("simt");
+    """d=256, F=2048, 512 tokens: every product takes the wgmma 3xTF32 GEMM ("tc") or the exact-fp32 FFMA kernel ("simt");
     three steps against the pinned oracle.  The ghost loss is ill-conditioned by construction (it divides by elements of
     (G - r)^2 / rcn + 1e-6): torch fp32 vs fp64 differ by 6e-4 on these gradients, the FFMA route stays within 3e-3, and the
     tensor-core route -- whose accumulation rounds toward zero, ~1e-5 on hidden_pre / sae_out -- within 6e-2 on the worst

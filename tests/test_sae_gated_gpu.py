@@ -1,6 +1,6 @@
 """Gated SAE step (vit_prisma/b200/sae_gated.py, csrc/sae_dense.cu pb_gated_*) against the reference fixtures
 (tests/golden/sae_gated_{g,h}.pt: autograd + torch.optim.Adam on the unmodified GatedSparseAutoencoder) and, at a size that takes
-the tcgen05 GEMMs, against the pinned oracle."""
+the wgmma GEMMs, against the pinned oracle."""
 import math
 
 import pytest
@@ -70,7 +70,7 @@ def test_gated_steps_match_reference_golden(tag):
 
 @pytest.mark.parametrize("impl", ["simt", "tc"])
 def test_gated_step_midsize_matches_oracle(impl):
-    """d=256, F=2048, 512 tokens: all seven products on the tcgen05 3xTF32 GEMM ("tc") or the exact FFMA kernel ("simt")."""
+    """d=256, F=2048, 512 tokens: all seven products on the wgmma 3xTF32 GEMM ("tc") or the exact FFMA kernel ("simt")."""
     d, F, rows, l1 = 256, 2048, 512, 2e-3
     g = torch.Generator().manual_seed(9)
     p = {"W_enc": torch.randn(d, F, generator=g) / math.sqrt(d), "W_dec": torch.randn(F, d, generator=g), "b_gate": 0.05 * torch.randn(F, generator=g),

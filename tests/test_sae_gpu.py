@@ -93,18 +93,6 @@ def test_fused_encode_topk_matches_float64_topk(rows, d, F, k, c_keep):
         assert eng.fallback_rows() <= max(2, rows // 50), f"{eng.fallback_rows()} of {rows} rows took the exact path on Gaussian data"
 
 
-@pytest.mark.parametrize("rows,d,F,k", [(300, 128, 2048, 8), (770, 768, 24576, 32), (1100, 100, 1280, 16)])
-def test_fused_encode_topk_cta_pair_kernel(rows, d, F, k, monkeypatch):
-    """The cta_group::2 candidate GEMM (256-token tiles across a CTA pair; ragged last tile, K tail) selects what the one-CTA kernel does."""
-    monkeypatch.setenv("PB_ENC_PAIR", "1")
-    eng, hp = _fused_case(rows, d, F, k, seed=rows + F)
-    _check_against_float64(eng, hp, k)
-    monkeypatch.setenv("PB_ENC_PAIR", "0")
-    eng1, _ = _fused_case(rows, d, F, k, seed=rows + F)
-    assert torch.equal(eng.idx, eng1.idx) and torch.equal(eng.val, eng1.val)
-    assert eng.fallback_rows() == eng1.fallback_rows()
-
-
 def test_fused_encode_topk_adversarial_rows_take_the_exact_path():
     """Cases the approximate pass cannot settle: constant rows (every value ties: lowest indices win), all winners inside one
     128-feature segment (more than c_keep of them: saturation), and rows with a huge norm next to tiny ones (loose error bound)."""
@@ -185,7 +173,7 @@ def test_train_steps_match_reference_golden(tag, impl):
 
 
 def test_engine_forward_matches_oracle_midsize():
-    """d=768, F=768*8, k=32, 512 tokens: above the size where the 128x128 tcgen05 tiles and the 24-per-thread TopK kick in."""
+    """d=768, F=768*8, k=32, 512 tokens: above the size where the 128x128 wgmma tiles and the 24-per-thread TopK kick in."""
     L = _L()
     from vit_prisma.b200.sae_engine import SaeStepEngine, unit_norm_rows_
     d, F, k, rows = 768, 768 * 8, 32, 512

@@ -1,14 +1,13 @@
 // attention_mma.cu -- fused hooked attention for d_head == 64 on warp-level tensor-core MMAs.
 //
-// Why not tcgen05 here: one head is a 50..257-token problem (S = Q K^T is 50x50 for ViT-B/32) and the op is bound by
-// the HBM traffic of its hook points (scores + pattern = 2*B*H*T*T elements written) -- a 128-row UMMA tile with a TMEM
+// Why not wgmma here: one head is a 50..257-token problem (S = Q K^T is 50x50 for ViT-B/32) and the op is bound by
+// the HBM traffic of its hook points (scores + pattern = 2*B*H*T*T elements written) -- a 64-row wgmma tile with a register
 // round trip would be mostly padding.  Warp-level mma.sync keeps S and P in registers between QK^T, softmax and PV.
 //
 // One CTA = one (batch, head) x one slab of NW*16 query rows; K, V (and the Q slab) of the head sit in shared memory,
 // row-major, copied in with 16-byte vectors (no conversion, no transposition on the way in).
 //   bf16 : mma.sync.m16n8k16 bf16 (fp32 accumulate); fragments come from ldmatrix (.trans for V, so the PV operand
-//          needs no transposed copy of V -- the transposing 2-byte stores of the first version cost 9.0M bank conflicts
-//          per launch, profiles/r01_attention_notes.md).
+//          needs no transposed copy of V -- the transposing 2-byte stores of a first version were bank-conflict bound).
 //   fp32 : mma.sync.m16n8k8 tf32 in 3 passes (x = hi + lo, hi = what the tensor core reads of x, lo = x - hi:
 //          lo*hi + hi*lo + hi*hi) -> fp32-grade products for the 1e-4 parity bar.
 // Hook points leave through a per-warp stage that holds the warp's 16 rows packed exactly as they lie in global memory
@@ -235,8 +234,9 @@ __global__ void __launch_bounds__(NW * 32) k_attention_mma(const T* __restrict__
     for (int c = 0; c < 4; ++c) {
       const int col = nt * 8 + 2 * t + (c & 1);
       const float x = acc[nt][c] - (c < 2 ? mx_lo : mx_hi);
-      // bf16: the pattern is rounded to 8 bits right after, MUFU.EX2's 2 ulp are invisible; fp32 keeps libdevice expf
-      const float e = col < Tn ? (BF ? __expf(x) : expf(x)) : 0.f;
+      // libdevice expf in both modes: with MUFU.EX2 (2 ulp) the bf16 pattern rounded the other way near half-ulp boundaries
+      // often enough to put hook_pattern / hook_z measurably further from the fp32 truth than the reference's own bf16 path
+      const float e = col < Tn ? expf(x) : 0.f;
       acc[nt][c] = e;
       if (c < 2) sum_lo += e; else sum_hi += e;
     }

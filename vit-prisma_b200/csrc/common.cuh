@@ -1,4 +1,4 @@
-// common.cuh -- shared helpers for libprisma_b200 (sm_100a only).
+// common.cuh -- shared helpers for libprisma_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -83,14 +83,14 @@ __device__ __forceinline__ void st4(bf16* p, const float (&v)[4]) {
   *reinterpret_cast<bf16x4*>(p) = t;
 }
 
-// tf32 split: hi = x with the 13 low mantissa bits cleared (what kind::tf32 consumes),
+// tf32 split: hi = x with the 13 low mantissa bits cleared (what tf32 wgmma consumes),
 // lo = x - hi (exact in fp32).
 __device__ __forceinline__ float tf32_trunc(float x) {
   return __uint_as_float(__float_as_uint(x) & 0xFFFFE000u);
 }
 // low plane of the 3xTF32 split: x - hi, itself rounded to the NEAREST tf32 so that the tensor core's truncating read of the
 // plane is exact.  A truncated lo loses up to 2^-20 |x| per element, always in the same direction, so the error of a K-term dot
-// product grows like K (measured 2.6e-5 at K = 3072); rounded, it is +-2^-21 |x| and averages out (profiles/r01_gemm_notes.md).
+// product grows like K; rounded, it is +-2^-21 |x| and averages out.
 __device__ __forceinline__ float tf32_lo(float x) {
   uint32_t r;
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x - tf32_trunc(x)));

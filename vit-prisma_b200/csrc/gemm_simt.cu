@@ -2,7 +2,7 @@
 //
 // Role: (1) the fp32 parity path (bit-for-bit fp32 products, fp32 accumulation -- what the
 // reference's CPU bmm computes up to summation order); (2) the shape-agnostic path for problems the
-// tcgen05 kernel (gemm_tc.cu) does not take (tiny d_model in unit tests, K not a multiple of the
+// wgmma kernel (gemm_tc.cu) does not take (tiny d_model in unit tests, K not a multiple of the
 // swizzle atom, unaligned leading dimensions); (3) the on-device cross-check for gemm_tc.cu.
 // 128x128x16 CTA tile, 256 threads, 8x8 register tile per thread (as 2x2 blocks of 4x4 so shared
 // loads are LDS.128 and global stores are 16 B), register-staged double buffering of the next k-slab.

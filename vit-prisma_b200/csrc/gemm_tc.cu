@@ -1,21 +1,20 @@
-// gemm_tc.cu -- tcgen05 / TMEM / TMA GEMM with the hooked epilogue (sm_100a).
+// gemm_tc.cu -- wgmma / TMA GEMM with the hooked epilogue (sm_90a).
 //
-//   out = A[M,K] @ B[N,K]^T, both operands K-major in HBM, fp32 accumulation in tensor memory.
+//   out = A[M,K] @ B[N,K]^T, both operands K-major in HBM, fp32 accumulation in registers.
 //
-// One CTA computes one 128 x BN output tile:
-//   warp 0   TMA producer : cp.async.bulk.tensor.2d (128B-swizzled boxes, one k-slab of 128 bytes per row)
-//                           into a STAGES-deep shared-memory ring, completion on "full" mbarriers;
-//   warp 1   MMA issuer   : one elected lane issues tcgen05.mma (M=128, N=BN, K=32 bytes per instruction)
-//                           straight from the swizzled tiles through shared-memory descriptors;
-//                           tcgen05.commit releases ring slots ("empty") and finally signals "accumulator ready";
-//   warps 2-5 epilogue    : tcgen05.ld (32 lanes x 32 columns per instruction) TMEM -> registers,
-//                           bias / activation / residual, hook-point spill to up to two destinations.
-// Two CTAs fit per SM in the bf16 configuration (3 x 32 KB ring + 128 TMEM columns each), so one CTA's
-// epilogue (the HBM-store-heavy part of a hooked GEMM) overlaps the other's mainloop.
+// Persistent kernel, one CTA per SM, 128 x 128 output tiles walked with a grid stride:
+//   warpgroup 0   TMA producer : one thread issues cp.async.bulk.tensor.2d (128B-swizzled boxes, one k-slab of 128 bytes per row)
+//                                into a STAGES-deep shared-memory ring, completion on "full" mbarriers;
+//   warpgroups 1-2 consumers   : each owns 64 rows of the tile and issues wgmma.mma_async m64n128 (32 bytes of K per
+//                                instruction) straight from the swizzled tiles through shared-memory descriptors; a slot is
+//                                handed back ("empty") once the wgmma group that read it has retired.  After the last k-slab
+//                                the accumulators go through a shared-memory transposer to the hooked epilogue (bias /
+//                                activation / residual, hook-point spill to up to two destinations) while the producer
+//                                already fills the ring with the next tile.
 //
 // Precision modes
-//   bf16  : kind::f16, bf16 operands.                       1 MMA per k-step
-//   tf32x3: kind::tf32 on fp32 operands split as x = hi + lo with hi = tf32_trunc(x) (the tensor core
+//   bf16  : wgmma .bf16, bf16 operands.                      1 MMA per k-step
+//   tf32x3: wgmma .tf32 on fp32 operands split as x = hi + lo with hi = tf32_trunc(x) (the tensor core
 //           ignores the 13 low mantissa bits, so the unsplit fp32 array *is* hi) and lo = x - hi stored
 //           separately:  A@B ~= Alo@Bhi + Ahi@Blo + Ahi@Bhi (lo*lo ~ 2^-22 relative is dropped).
 //           3 MMAs per k-step into the same accumulator -> fp32-grade products for the 1e-4 parity bar.
@@ -26,175 +25,6 @@
 #include "tc_common.cuh"
 
 namespace {
-
-template <typename T, int NPASS, int BN, int STAGES>
-__global__ void __launch_bounds__(TC_THREADS) k_gemm_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                                                        const __grid_constant__ CUtensorMap tmAlo,
-                                                        const __grid_constant__ CUtensorMap tmBlo, int K, EpiParams ep) {
-  using C = TcCfg<T, NPASS, BN, STAGES>;
-  constexpr int KIND = sizeof(T) == 2 ? 0 : 1;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t ring = (smem_u32(smem_raw) + 1023u) & ~1023u;  // SWIZZLE_128B tiles need 1024 B alignment
-  const uint32_t bar_base = ring + C::RING_BYTES;
-  // barrier block: full[STAGES] | empty[STAGES] | tmem_full | tmem_ptr(u32)
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  const uint32_t tmem_full_bar = bar_base + 8u * (2 * STAGES);
-  const uint32_t tmem_ptr_addr = bar_base + 8u * (2 * STAGES + 1);
-  volatile uint32_t* tmem_ptr_generic = reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_ptr_addr - smem_u32(smem_raw)));
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int m0 = blockIdx.y * TC_BM, n0 = blockIdx.x * BN;
-  const int num_kb = (K + C::BK - 1) / C::BK;
-
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&tmA);
-    prefetch_tmap(&tmB);
-    if (NPASS == 3) { prefetch_tmap(&tmAlo); prefetch_tmap(&tmBlo); }
-    for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 1); }
-    mbar_init(tmem_full_bar, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) {  // TMEM allocation: one warp, BN fp32 columns x 128 lanes
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_ptr_addr), "r"((uint32_t)BN) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_generic;
-
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (lane == 0) {
-      for (int kb = 0; kb < num_kb; ++kb) {
-        const int s = kb % STAGES;
-        const uint32_t ph = (kb / STAGES) & 1;
-        mbar_wait(empty_bar(s), ph ^ 1);
-        mbar_expect_tx(full_bar(s), C::STAGE_BYTES);
-        const uint32_t sa = ring + s * C::STAGE_BYTES;
-        const int kc = kb * C::BK;
-        tma_load_2d(sa, &tmA, full_bar(s), kc, m0);
-        if (NPASS == 3) tma_load_2d(sa + C::A_BYTES, &tmAlo, full_bar(s), kc, m0);
-        const uint32_t sb = sa + C::NOP * C::A_BYTES;
-        tma_load_2d(sb, &tmB, full_bar(s), kc, n0);
-        if (NPASS == 3) tma_load_2d(sb + C::B_BYTES, &tmBlo, full_bar(s), kc, n0);
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      for (int kb = 0; kb < num_kb; ++kb) {
-        const int s = kb % STAGES;
-        const uint32_t ph = (kb / STAGES) & 1;
-        mbar_wait(full_bar(s), ph);
-        tc_fence_after();
-        const uint32_t sa = ring + s * C::STAGE_BYTES;
-        const uint32_t sb = sa + C::NOP * C::A_BYTES;
-#pragma unroll
-        for (int k = 0; k < 128 / C::UMMA_K_BYTES; ++k) {
-          const uint32_t koff = k * C::UMMA_K_BYTES;
-          const uint64_t a_hi = make_smem_desc(sa + koff);
-          const uint64_t b_hi = make_smem_desc(sb + koff);
-          const uint32_t first = (kb | k) != 0 ? 1u : 0u;
-          if (NPASS == 3) {
-            const uint64_t a_lo = make_smem_desc(sa + C::A_BYTES + koff);
-            const uint64_t b_lo = make_smem_desc(sb + C::B_BYTES + koff);
-            tc_mma<KIND>(tmem_base, a_lo, b_hi, C::IDESC, first);
-            tc_mma<KIND>(tmem_base, a_hi, b_lo, C::IDESC, 1u);
-            tc_mma<KIND>(tmem_base, a_hi, b_hi, C::IDESC, 1u);
-          } else {
-            tc_mma<KIND>(tmem_base, a_hi, b_hi, C::IDESC, first);
-          }
-        }
-        tc_commit(empty_bar(s));  // slot reusable once these MMAs have read it
-      }
-      tc_commit(tmem_full_bar);  // accumulator complete
-    }
-  } else {
-    // ===================== epilogue =====================
-    // TMEM hands each thread one accumulator ROW (32 consecutive columns per tcgen05.ld); storing from that layout
-    // makes every warp store touch 32 different rows (measured: ~190 GB/s).  So each 32x32 chunk is transposed through
-    // shared memory (the operand ring is idle once "accumulator ready" fired) and written row by row: one warp
-    // instruction = 32 consecutive columns of one row = one full 128-byte line (fp32), bias / activation / residual
-    // applied in that coalesced layout, residual reads coalesced too.
-    const int quarter = warp & 3;  // TMEM lane quarter this warp may access
-    mbar_wait(tmem_full_bar, 0);
-    tc_fence_after();
-    float* stage = reinterpret_cast<float*>(smem_raw + (ring - smem_u32(smem_raw))) + (warp - 2) * (32 * 33);
-    const T* bias = (const T*)ep.bias;
-    const int row0 = m0 + quarter * 32;
-    const int nrows = min(32, ep.M - row0);
-#pragma unroll 1
-    for (int c = 0; c < BN / 32; ++c) {
-      uint32_t r[32];
-      tmem_ld32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(c * 32), r);
-      tmem_ld_wait();
-#pragma unroll
-      for (int j = 0; j < 32; ++j) stage[lane * 33 + j] = __uint_as_float(r[j]);
-      __syncwarp();
-      const int col = n0 + c * 32 + lane;
-      if (col < ep.N && nrows > 0) {
-        const bool has_bias = bias != nullptr;
-        const float bv = has_bias ? ld_as_float(bias + col) : 0.f;
-        T* o0 = nullptr;
-        if (ep.n_split > 1) {
-          const int blk = col / ep.split_n;
-          o0 = (T*)(blk == 0 ? ep.out_split[0] : blk == 1 ? ep.out_split[1] : blk == 2 ? ep.out_split[2] : ep.out_split[3]) + (col - blk * ep.split_n);
-        } else if (ep.out0) {
-          o0 = (T*)ep.out0 + col;
-        }
-        if (o0) o0 += (int64_t)row0 * ep.ld0;
-        T* o1 = ep.out1 ? (T*)ep.out1 + (int64_t)row0 * ep.ld1 + col : nullptr;
-        float* o1lo = ep.out1_lo ? ep.out1_lo + (int64_t)row0 * ep.ld1 + col : nullptr;
-        const T* res = ep.residual ? (const T*)ep.residual + (int64_t)row0 * ep.ldr + col : nullptr;
-        for (int rr = 0; rr < nrows; ++rr) {
-          const float a = stage[rr * 33 + lane];
-          const float v = has_bias ? round_to<T>(round_to<T>(a) + bv) : round_to<T>(a);
-          if (o0) { st_from_float(o0, v); o0 += ep.ld0; }
-          if (o1) {
-            float o;
-            if (res) { o = ld_as_float(res) + v; res += ep.ldr; }
-            else o = apply_act(v, ep.act);
-            st_from_float(o1, o);
-            o1 += ep.ld1;
-            if (o1lo) { *o1lo = tf32_lo(o); o1lo += ep.ld1; }
-          }
-        }
-      }
-      __syncwarp();
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)BN) : "memory");
-  }
-}
-
-// =====================================================================================================
-// v2: persistent kernel, one CTA per SM, 128 x BN tiles (BN = 256 for bf16), double-buffered accumulators.
-//
-// Measured on v1 (128x128 tile per CTA, profiles/r01_gemm_notes.md): the mainloop is bound by L2->SM operand
-// bandwidth (a 128x128 tile moves 32 KB per 1 M MACs: 64 flop/B against ~12 TB/s of L2), and the epilogue of a
-// hooked GEMM (two full-size outputs + GELU) costs as much as the mainloop and only overlaps by luck of co-residency.
-// v2 therefore (a) widens the tile to 128x256 (85 flop/B), (b) keeps TWO accumulators in TMEM (2 x BN columns of 512)
-// so that tcgen05.mma fills one while the epilogue drains the other, (c) spreads the epilogue over 8 warps
-// (two per TMEM lane quarter, each owning half of the columns), (d) walks tiles n-fastest so the CTAs of a wave share
-// A rows in L2 while the whole weight matrix stays L2-resident.
-
-template <typename T, int NPASS, int BN, int STAGES, int NEPI>
-struct Tc2Cfg {
-  using Base = TcCfg<T, NPASS, BN, STAGES>;
-  static constexpr int THREADS = 64 + NEPI * 32;
-  static constexpr int EPI_WARP_FLOATS = sizeof(T) == 2 ? 32 * 33 : 32 * 36;
-  static constexpr int EPI_STAGE_BYTES = NEPI * EPI_WARP_FLOATS * 4;   // 32x33 fp32 transposer (tail path) / 32 rows x 144 B vector stage
-  static constexpr int SMEM_BYTES = Base::RING_BYTES + EPI_STAGE_BYTES + 1024 + 256;
-  static constexpr int TMEM_COLS = 2 * BN;
-  static_assert(TMEM_COLS <= 512 && (TMEM_COLS & (TMEM_COLS - 1)) == 0, "TMEM columns must be a power of two <= 512");
-  static_assert(SMEM_BYTES <= 232448, "shared memory budget exceeded");
-};
 
 template <typename T>
 __device__ __forceinline__ void epi_rows_scalar(const EpiParams& ep, const float* stage, int lane, int row0, int nrows, int col) {
@@ -238,12 +68,12 @@ __device__ __forceinline__ void ld2(const bf16* p, float& a, float& b) {
 
 // GELU(x) = x/2 (1 + erf(x/sqrt2)) with erf from Abramowitz-Stegun 7.1.26 (|erf error| <= 1.5e-7, branch-free, one
 // MUFU.EX2 + one MUFU.RCP): the epilogue of the MLP-in GEMM evaluates it B*T*d_mlp times per block and was issue-bound
-// on libdevice's branchy erff (profiles/r01_gemm_notes.md).  Absolute error of the result <= 0.75e-7 |x|.
+// on libdevice's branchy erff.  Absolute error of the result <= 0.75e-7 |x|.
 __device__ __forceinline__ float mufu_rcp(float x) { float r; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x)); return r; }
 __device__ __forceinline__ float mufu_ex2(float x) { float r; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x)); return r; }
 __device__ __forceinline__ float gelu_fast(float x) {
   // single MUFU.RCP / MUFU.EX2, no IEEE fix-up branches: __frcp_rn's slow path put a BSSY/BSYNC pair around every element,
-  // which serialised the 32 unrolled evaluations (0.265 ms -> see profiles/r01_gemm_notes.md)
+  // which serialised the 32 unrolled evaluations
   const float ax = fabsf(x) * 0.70710678118654752440f;
   const float t = mufu_rcp(fmaf(0.3275911f, ax, 1.f));
   float p = fmaf(t, 1.061405429f, -1.453152027f);
@@ -322,12 +152,12 @@ __device__ __forceinline__ void epi_rows_pair(const EpiParams& ep, const float* 
 #undef PB_EPI
 }
 
-// ---- v3 epilogue: arithmetic in TMEM's native layout, shared memory only as a 16-byte-vector transposer ----------------
-// tcgen05.ld gives thread t row t of a 32x32 chunk.  Bias / rounding / GELU / residual are applied right there (constant
+// ---- row-per-lane epilogue: shared memory only as a 16-byte-vector transposer --------------------------------------
+// The caller gives thread t row t of a 32x32 chunk.  Bias / rounding / GELU / residual are applied right there (constant
 // register indices, no per-element address arithmetic); the packed results are written as the thread's row into a padded
 // stage (row stride 32*sizeof(T)+16 B: conflict-free for 128-bit accesses) and copied out with 16 B loads/stores where
 // consecutive lanes cover consecutive 16 B of a row.  ~20 instructions per element against ~56 for the per-element walk
-// (profiles/r01_gemm_notes.md), and every global access is a full 16 B vector of a contiguous row segment.
+// and every global access is a full 16 B vector of a contiguous row segment.
 template <typename T> struct EpiStage {
   static constexpr int VPR = 32 * (int)sizeof(T) / 16;        // 16-byte vectors per 32-column row: 4 (bf16) / 8 (fp32)
   static constexpr int ROW_BYTES = 32 * (int)sizeof(T) + 16;
@@ -457,60 +287,77 @@ __device__ __forceinline__ void epi_chunk_vec(const EpiParams& ep, const uint32_
   }
 }
 
-template <typename T, int NPASS, int BN, int STAGES, int NEPI>
-__global__ void __launch_bounds__(64 + NEPI * 32, 1)
-k_gemm_tc2(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmAlo,
-           const __grid_constant__ CUtensorMap tmBlo, int K, EpiParams ep, int num_m_tiles, int num_n_tiles, int m_fast) {
-  using C = TcCfg<T, NPASS, BN, STAGES>;
-  using C2 = Tc2Cfg<T, NPASS, BN, STAGES, NEPI>;
-  // raster order of the persistent tile walk: the ~148 tiles in flight share one operand through L2 and stream the other.
+
+// Epilogue transposer: per consumer warp one 32 x 32 fp32 block (row stride 33, conflict-free when a lane reads its row),
+// sized for the 16-byte-vector stage of epi_chunk_vec (32 rows x 144 B) that reuses it once the block is in registers.
+constexpr int EPI_WARP_BYTES = 32 * 36 * 4;
+template <typename T, int NPASS, int STAGES>
+struct TcSmem {
+  using C = TcCfg<T, NPASS, STAGES>;
+  static constexpr int EPI_BYTES = 8 * EPI_WARP_BYTES;
+  static constexpr int SMEM_BYTES = C::RING_BYTES + EPI_BYTES + 1024 /*alignment slack*/ + 256 /*barriers*/;
+  static_assert(SMEM_BYTES <= 232448, "shared memory budget exceeded");
+};
+
+template <typename T, int NPASS>
+__device__ __forceinline__ void wgmma_step(float (&acc)[64], uint32_t sa, uint32_t sb, uint32_t koff, uint32_t a_lo_off, uint32_t b_lo_off,
+                                           uint32_t first) {
+  const uint64_t a_hi = make_smem_desc(sa + koff);
+  const uint64_t b_hi = make_smem_desc(sb + koff);
+  if (sizeof(T) == 2) {
+    wgmma_bf16_n128(acc, a_hi, b_hi, first);
+  } else if (NPASS == 3) {
+    wgmma_tf32_n128(acc, make_smem_desc(sa + a_lo_off + koff), b_hi, first);
+    wgmma_tf32_n128(acc, a_hi, make_smem_desc(sb + b_lo_off + koff), 1u);
+    wgmma_tf32_n128(acc, a_hi, b_hi, 1u);
+  } else {
+    wgmma_tf32_n128(acc, a_hi, b_hi, first);
+  }
+}
+
+template <typename T, int NPASS, int STAGES>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+k_gemm_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmAlo,
+          const __grid_constant__ CUtensorMap tmBlo, int K, EpiParams ep, int num_m_tiles, int num_n_tiles, int m_fast) {
+  using C = TcCfg<T, NPASS, STAGES>;
+  // raster order of the persistent tile walk: the ~132 tiles in flight share one operand through L2 and stream the other.
   // n-fastest (default) streams A once and wants B (the weights) L2-resident; m_fast streams B once and keeps A resident --
-  // the SAE encoder (A = 4096 tokens, B = 24576 x 768 dictionary, 151 MB with its lo plane) needs the latter.
+  // a large dictionary against a few thousand tokens (the SAE products) needs the latter.
   auto tile_m = [&](int tile) { return m_fast ? tile % num_m_tiles : tile / num_n_tiles; };
   auto tile_n = [&](int tile) { return m_fast ? tile / num_m_tiles : tile % num_n_tiles; };
-  constexpr int KIND = sizeof(T) == 2 ? 0 : 1;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem0 = smem_u32(smem_raw);
-  const uint32_t ring = (smem0 + 1023u) & ~1023u;
+  const uint32_t ring = (smem0 + 1023u) & ~1023u;     // SWIZZLE_128B tiles need 1024 B alignment
   const uint32_t epi_stage = ring + C::RING_BYTES;
-  const uint32_t bar_base = epi_stage + C2::EPI_STAGE_BYTES;
+  const uint32_t bar_base = epi_stage + 8 * EPI_WARP_BYTES;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * STAGES + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * STAGES + 2 + a); };
-  const uint32_t tmem_ptr_addr = bar_base + 8u * (2 * STAGES + 4);
-  volatile uint32_t* tmem_ptr_generic = reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_ptr_addr - smem0));
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = warp >> 2;
   const int num_kb = (K + C::BK - 1) / C::BK;
   const int num_tiles = num_m_tiles * num_n_tiles;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB);
     if (NPASS == 3) { prefetch_tmap(&tmAlo); prefetch_tmap(&tmBlo); }
-    for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(tfull_bar(a), 1); mbar_init(tempty_bar(a), NEPI); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 2); }   // empty: one arrival per consumer warpgroup
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_ptr_addr), "r"((uint32_t)C2::TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_generic;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (wg == 0) {
+    // ===================== TMA producer =====================
+    reg_dealloc<40>();
+    if (threadIdx.x == 0) {
       uint32_t it = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int m0 = tile_m(tile) * TC_BM, n0 = tile_n(tile) * BN;
+        const int m0 = tile_m(tile) * TC_BM, n0 = tile_n(tile) * TC_BN;
         for (int kb = 0; kb < num_kb; ++kb, ++it) {
           const int s = it % STAGES;
           const uint32_t ph = (it / STAGES) & 1;
-          mbar_wait(empty_bar(s), ph ^ 1);
+          mbar_wait<false>(empty_bar(s), ph ^ 1);
           mbar_expect_tx(full_bar(s), C::STAGE_BYTES);
           const uint32_t sa = ring + s * C::STAGE_BYTES;
           const int kc = kb * C::BK;
@@ -522,152 +369,124 @@ k_gemm_tc2(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      uint32_t it = 0;
-      int li = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++li) {
-        const int ab = li & 1;
-        const uint32_t aph = (li >> 1) & 1;
-        mbar_wait(tempty_bar(ab), aph ^ 1);      // epilogue has drained this accumulator (first two uses pass at once)
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(ab * BN);
-        for (int kb = 0; kb < num_kb; ++kb, ++it) {
-          const int s = it % STAGES;
-          const uint32_t ph = (it / STAGES) & 1;
-          mbar_wait(full_bar(s), ph);
-          tc_fence_after();
-          const uint32_t sa = ring + s * C::STAGE_BYTES;
-          const uint32_t sb = sa + C::NOP * C::A_BYTES;
-#pragma unroll
-          for (int k = 0; k < 128 / C::UMMA_K_BYTES; ++k) {
-            const uint32_t koff = k * C::UMMA_K_BYTES;
-            const uint64_t a_hi = make_smem_desc(sa + koff);
-            const uint64_t b_hi = make_smem_desc(sb + koff);
-            const uint32_t first = (kb | k) != 0 ? 1u : 0u;
-            if (NPASS == 3) {
-              const uint64_t a_lo = make_smem_desc(sa + C::A_BYTES + koff);
-              const uint64_t b_lo = make_smem_desc(sb + C::B_BYTES + koff);
-              tc_mma<KIND>(d_tmem, a_lo, b_hi, C::IDESC, first);
-              tc_mma<KIND>(d_tmem, a_hi, b_lo, C::IDESC, 1u);
-              tc_mma<KIND>(d_tmem, a_hi, b_hi, C::IDESC, 1u);
-            } else {
-              tc_mma<KIND>(d_tmem, a_hi, b_hi, C::IDESC, first);
-            }
-          }
-          tc_commit(empty_bar(s));
-        }
-        tc_commit(tfull_bar(ab));
-      }
-    }
-  } else {
-    const int e = warp - 2;                      // 0 .. NEPI-1
-    const int quarter = warp & 3;                // TMEM lane quarter this warp may read
-    constexpr int CPW = BN / (NEPI / 4);         // columns per epilogue warp
-    const int cbase = (e / 4) * CPW;
-    float* stage = reinterpret_cast<float*>(smem_raw + (epi_stage - smem0)) + e * C2::EPI_WARP_FLOATS;
-    int li = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++li) {
-      const int m0 = tile_m(tile) * TC_BM, n0 = tile_n(tile) * BN;
-      const int ab = li & 1;
-      const uint32_t aph = (li >> 1) & 1;
-      mbar_wait(tfull_bar(ab), aph);
-      tc_fence_after();
-      const int row0 = m0 + quarter * 32;
-      const int nrows = min(32, ep.M - row0);
-#pragma unroll 1
-      for (int c = 0; c < CPW / 32; ++c) {
-        uint32_t r[32];
-        tmem_ld32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(ab * BN + cbase + c * 32), r);
-        tmem_ld_wait();
-        if (c == CPW / 32 - 1) {                 // last read of this accumulator: hand it back to the MMA warp early
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(tempty_bar(ab));
-        }
-        const int col0 = n0 + cbase + c * 32;
-        if (ep.vec16_ok && col0 + 32 <= ep.N) {     // whole chunk inside the matrix: native-layout epilogue
-          if (nrows > 0) epi_chunk_vec<T>(ep, r, reinterpret_cast<uint8_t*>(stage), lane, row0, nrows, col0);
-        } else {                                     // ragged edge / unaligned operands: per-element walk
-#pragma unroll
-          for (int j = 0; j < 32; ++j) stage[lane * 33 + j] = __uint_as_float(r[j]);
-          __syncwarp();
-          if (nrows > 0) {
-            if (ep.vec_ok) epi_rows_pair<T>(ep, stage, lane, row0, nrows, col0);
-            else if (col0 + lane < ep.N) epi_rows_scalar<T>(ep, stage, lane, row0, nrows, col0 + lane);
-          }
-          __syncwarp();
-        }
-      }
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)C2::TMEM_COLS) : "memory");
+  // ===================== consumers: warpgroup c owns rows [64 c, 64 c + 64) of each tile =====================
+  reg_alloc<232>();
+  const int c = wg - 1;
+  const int wq = warp & 3;                 // warp inside the warpgroup
+  const int tid = threadIdx.x & 127;
+  uint8_t* stage_wg = smem_raw + (epi_stage - smem0) + c * 4 * EPI_WARP_BYTES;
+  float* region = reinterpret_cast<float*>(stage_wg + wq * EPI_WARP_BYTES);
+  // bf16: every 64-wide k-slab goes into a fresh wgmma accumulator that is then added into `acc` with FADD.  The tensor core's own
+  // fp32 accumulation over the whole K chain rounded the bf16 outputs measurably further from the exact sum than the reference's
+  // fp32 GEMM.  The slab's group is waited for at once; the other consumer warpgroup's MMAs keep the tensor core busy meanwhile.
+  constexpr bool PROMOTE = sizeof(T) == 2;
+  float acc[64], part[PROMOTE ? 64 : 1];
+  uint32_t it = 0;
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    const int m0 = tile_m(tile) * TC_BM, n0 = tile_n(tile) * TC_BN;
+    int prev_s = -1;
+    if constexpr (PROMOTE) {
+#pragma unroll
+      for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    }
+    for (int kb = 0; kb < num_kb; ++kb, ++it) {
+      const int s = it % STAGES;
+      const uint32_t ph = (it / STAGES) & 1;
+      mbar_wait<false>(full_bar(s), ph);
+      const uint32_t sa = ring + s * C::STAGE_BYTES + c * 64 * 128;       // this warpgroup's 64 rows of A
+      const uint32_t sb = ring + s * C::STAGE_BYTES + C::NOP * C::A_BYTES;
+      wgmma_fence();
+      if constexpr (PROMOTE) {
+#pragma unroll
+        for (int k = 0; k < C::KSTEPS; ++k) wgmma_step<T, NPASS>(part, sa, sb, 32u * k, C::A_BYTES, C::B_BYTES, k != 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_acc(part);
+        if (tid == 0) mbar_arrive(empty_bar(s));
+#pragma unroll
+        for (int i = 0; i < 64; ++i) acc[i] += part[i];
+      } else {
+#pragma unroll
+        for (int k = 0; k < C::KSTEPS; ++k)
+          wgmma_step<T, NPASS>(acc, sa, sb, 32u * k, C::A_BYTES, C::B_BYTES, (kb | k) != 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();                      // the group of the previous k-slab has retired: its slot may be refilled
+        if (prev_s >= 0 && tid == 0) mbar_arrive(empty_bar(prev_s));
+        prev_s = s;
+      }
+    }
+    if constexpr (!PROMOTE) {
+      wgmma_wait<0>();
+      wgmma_fence_acc(acc);
+      if (tid == 0) mbar_arrive(empty_bar(prev_s));
+    }
+
+    // ---- epilogue, 64 columns at a time.  Accumulator element i of thread (warp w, lane l) is row 16 w + l / 4 + 8 ((i >> 1) & 1),
+    // column 8 (i >> 2) + 2 (l % 4) + (i & 1) of the warpgroup's 64 x 128 block.  Warp q of the warpgroup then takes the 32 x 32
+    // block q (rows 32 (q & 1) .., columns 32 (q >> 1) .. of the 64-column half) with one row per lane.
+#pragma unroll
+    for (int half = 0; half < 2; ++half) {
+#pragma unroll
+      for (int i = 32 * half; i < 32 * half + 32; ++i) {
+        const int r = 16 * wq + (lane >> 2) + 8 * ((i >> 1) & 1);
+        const int col = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1) - 64 * half;
+        float* dst = reinterpret_cast<float*>(stage_wg + ((r >> 5) | ((col >> 5) << 1)) * EPI_WARP_BYTES);
+        dst[(r & 31) * 33 + (col & 31)] = acc[i];
+      }
+      wg_sync(1 + c);
+      const int row0 = m0 + 64 * c + 32 * (wq & 1);
+      const int nrows = min(32, ep.M - row0);
+      const int col0 = n0 + 64 * half + 32 * (wq >> 1);
+      if (nrows > 0 && col0 < ep.N) {
+        if (ep.vec16_ok && col0 + 32 <= ep.N) {     // whole chunk inside the matrix: row-per-lane epilogue with 16-byte stores
+          uint32_t r[32];
+#pragma unroll
+          for (int j = 0; j < 32; ++j) r[j] = __float_as_uint(region[lane * 33 + j]);
+          __syncwarp();
+          epi_chunk_vec<T>(ep, r, reinterpret_cast<uint8_t*>(region), lane, row0, nrows, col0);
+        } else {                                     // ragged edge / unaligned operands: per-element walk
+          if (ep.vec_ok) epi_rows_pair<T>(ep, region, lane, row0, nrows, col0);
+          else if (col0 + lane < ep.N) epi_rows_scalar<T>(ep, region, lane, row0, nrows, col0 + lane);
+        }
+      }
+      wg_sync(1 + c);                                // every warp is done with the blocks before the next half lands in them
+    }
   }
 }
 
 // ---------------------------------------------------------------- host side
-template <typename T, int NPASS, int BN, int STAGES>
+template <typename T, int NPASS, int STAGES>
 int launch_tc(const PbGemm* g, cudaStream_t st) {
-  using C = TcCfg<T, NPASS, BN, STAGES>;
+  using S = TcSmem<T, NPASS, STAGES>;
   CUtensorMap tmA, tmB, tmAlo, tmBlo;
   PB_TRY(make_map(&tmA, g->A, g->dtype, g->M, g->K, g->lda, TC_BM));
-  PB_TRY(make_map(&tmB, g->B, g->dtype, g->N, g->K, g->ldb, BN));
+  PB_TRY(make_map(&tmB, g->B, g->dtype, g->N, g->K, g->ldb, TC_BN));
   if (NPASS == 3) {
     PB_TRY(make_map(&tmAlo, g->A_lo, g->dtype, g->M, g->K, g->lda, TC_BM));
-    PB_TRY(make_map(&tmBlo, g->B_lo, g->dtype, g->N, g->K, g->ldb, BN));
+    PB_TRY(make_map(&tmBlo, g->B_lo, g->dtype, g->N, g->K, g->ldb, TC_BN));
   } else {
     tmAlo = tmA;
     tmBlo = tmB;
   }
-  auto kern = k_gemm_tc<T, NPASS, BN, STAGES>;
+  auto kern = k_gemm_tc<T, NPASS, STAGES>;
   static bool attr_done = false;  // per instantiation
   if (!attr_done) {
-    PB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
+    PB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::SMEM_BYTES));
     attr_done = true;
   }
   EpiParams ep = pb_make_epi(g);
-  dim3 grid((g->N + BN - 1) / BN, (g->M + TC_BM - 1) / TC_BM);
-  kern<<<grid, TC_THREADS, C::SMEM_BYTES, st>>>(tmA, tmB, tmAlo, tmBlo, g->K, ep);
-  PB_LAUNCH_CHECK();
-  return PB_OK;
-}
-
-template <typename T, int NPASS, int BN, int STAGES, int NEPI>
-int launch_tc2(const PbGemm* g, cudaStream_t st) {
-  using C2 = Tc2Cfg<T, NPASS, BN, STAGES, NEPI>;
-  CUtensorMap tmA, tmB, tmAlo, tmBlo;
-  PB_TRY(make_map(&tmA, g->A, g->dtype, g->M, g->K, g->lda, TC_BM));
-  PB_TRY(make_map(&tmB, g->B, g->dtype, g->N, g->K, g->ldb, BN));
-  if (NPASS == 3) {
-    PB_TRY(make_map(&tmAlo, g->A_lo, g->dtype, g->M, g->K, g->lda, TC_BM));
-    PB_TRY(make_map(&tmBlo, g->B_lo, g->dtype, g->N, g->K, g->ldb, BN));
-  } else {
-    tmAlo = tmA;
-    tmBlo = tmB;
-  }
-  auto kern = k_gemm_tc2<T, NPASS, BN, STAGES, NEPI>;
-  static bool attr_done = false;
-  if (!attr_done) {
-    PB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C2::SMEM_BYTES));
-    attr_done = true;
-  }
-  EpiParams ep = pb_make_epi(g);
-  const int num_m = (g->M + TC_BM - 1) / TC_BM, num_n = (g->N + BN - 1) / BN;
+  const int num_m = (g->M + TC_BM - 1) / TC_BM, num_n = (g->N + TC_BN - 1) / TC_BN;
   int grid = pb_sm_count();
   if (grid > num_m * num_n) grid = num_m * num_n;
   const size_t planes = NPASS > 1 ? 2 : 1;
   const size_t a_bytes = (size_t)g->M * g->K * sizeof(T) * planes, b_bytes = (size_t)g->N * g->K * sizeof(T) * planes;
-  const int m_fast = (b_bytes > ((size_t)48 << 20) && a_bytes < b_bytes) ? 1 : 0;
-  kern<<<grid, C2::THREADS, C2::SMEM_BYTES, st>>>(tmA, tmB, tmAlo, tmBlo, g->K, ep, num_m, num_n, m_fast);
+  const int m_fast = (b_bytes > ((size_t)24 << 20) && a_bytes < b_bytes) ? 1 : 0;   // B no longer fits half of the 50 MB L2
+  kern<<<grid, TC_THREADS, S::SMEM_BYTES, st>>>(tmA, tmB, tmAlo, tmBlo, g->K, ep, num_m, num_n, m_fast);
   PB_LAUNCH_CHECK();
   return PB_OK;
 }
-
-#include "gemm_tc_pair.cuh"
 
 }  // namespace
 
@@ -690,24 +509,7 @@ int pb_gemm_tc(const PbGemm* g, cudaStream_t st) {
                  g->dtype, (long long)g->lda, (long long)g->ldb);
     return PB_EUNSUPPORTED;
   }
-  static int variant = -1;  // PB_GEMM_TC_VARIANT=1 forces the one-tile-per-CTA kernel (A/B measurements)
-  if (variant < 0) { const char* e = getenv("PB_GEMM_TC_VARIANT"); variant = e ? atoi(e) : 0; }
-  // CTA pairs (cta_group::2, 256 x 256 per pair, gemm_tc_pair.cuh): each SM loads half of the B tile, which is what the persistent
-  // single-CTA kernel was waiting for.  Measured on the ViT-B/32 shapes at M = 25600 (profiles/r02_gemm_notes.md):
-  //   3xTF32  +6 .. +18 % on every shape and epilogue   -> default whenever M, N >= 256
-  //   bf16    +1 .. +9 % with one output / a residual epilogue, -5 % with the two-output GELU epilogue (epilogue-bound: the pair
-  //           couples two epilogues to one accumulator hand-back)  -> default except for activation epilogues
-  // PB_GEMM_TC_VARIANT: 0 = this policy, 1 = one tile per CTA (v1), 2 = fp32 wide single-CTA tile, 3 = pairs everywhere, 4 = never pairs.
-  const bool pair_ok = g->N >= 256 && g->M >= 256 && variant != 1 && variant != 2 && variant != 4;
-  if (g->dtype == PB_BF16) {
-    const bool act_epilogue = g->out1 && !g->residual && g->act != PB_ACT_NONE;
-    if (pair_ok && (variant == 3 || !act_epilogue)) return launch_tc2_pair<bf16, 1, 256, 6, 8>(g, st);
-    if (variant != 1 && g->N >= 256) return launch_tc2<bf16, 1, 256, 4, 8>(g, st);
-    if (variant != 1 && g->N >= 128) return launch_tc2<bf16, 1, 128, 4, 4>(g, st);
-    return launch_tc<bf16, 1, 128, 3>(g, st);
-  }
-  if (variant == 2 && g->N >= 256) return launch_tc2<float, 3, 256, 2, 4>(g, st);   // wider tile, shallower ring (A/B)
-  if (pair_ok) return launch_tc2_pair<float, 3, 256, 3, 4>(g, st);
-  if (variant != 1) return launch_tc2<float, 3, 128, 3, 4>(g, st);
-  return launch_tc<float, 3, 128, 3>(g, st);
+  // ring depth: bf16 4 x 32 KB, 3xTF32 (hi + lo planes of both operands) 2 x 64 KB; the 36 KB epilogue transposer sits beside it
+  if (g->dtype == PB_BF16) return launch_tc<bf16, 1, 4>(g, st);
+  return launch_tc<float, 3, 2>(g, st);
 }

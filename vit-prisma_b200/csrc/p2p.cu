@@ -1,4 +1,4 @@
-// p2p.cu -- data-parallel SAE training over NVLink 5 / NVSwitch peer memory, no NCCL on the data path.
+// p2p.cu -- data-parallel SAE training over NVLink 4 / NVSwitch peer memory, no NCCL on the data path.
 //
 // One process per GPU (torchrun).  Buffers that peers must see (gradients, parameters, a few small vectors and the
 // barrier flags) are cudaMalloc'd here and exported with CUDA IPC handles; the host side (vit_prisma/b200/p2p.py)

@@ -1,5 +1,5 @@
 // sae.cu -- TopK sparse-autoencoder forward / training step (reference sae/sae.py:32-645,
-// sae/train_sae.py:278-411) as HBM-bound sm_100a kernels around one tensor-core GEMM.
+// sae/train_sae.py:278-411) as HBM-bound sm_90a kernels around one tensor-core GEMM.
 //
 // Data layout in HBM (all fp32, F = d_sae, d = d_in, Bt = tokens per step):
 //   W_encT [F][d]   encoder, stored feature-major (the nn.Parameter W_enc [d,F] is a transposed VIEW of it):
@@ -444,7 +444,7 @@ __global__ void __launch_bounds__(256) k_sae_grads(const int* __restrict__ off, 
 #pragma unroll
   for (int i = 0; i < CHUNKS; ++i) bd[i][0] = bd[i][1] = bd[i][2] = bd[i][3] = 0.f;
   // dynamic queue: list lengths vary (mean Bt*k/F, long tail), and with a static feature -> warp map the CTA waited at its final
-  // barrier for its slowest warp (9.9 barrier-stall cycles per issue, profiles/r02_sae_step_ncu_summary.txt)
+  // barrier for its slowest warp
   for (;;) {
     int fbase = 0;
     if (lane == 0) fbase = atomicAdd(&work->next_f, SAE_CLAIM);
@@ -486,7 +486,7 @@ __global__ void __launch_bounds__(256) k_sae_grads(const int* __restrict__ off, 
     // (rank by counting: entries are distinct; token order makes the fp32 sums deterministic), then lane i loads ITS entry's
     // activation / d(pre-activation) / token row index.  The accumulation loop below only shuffles those out of registers, so the
     // row gathers of consecutive entries are independent loads in flight together.  (Before: entry -> val / dval -> rows was a chain
-    // of three dependent L2 round trips PER PAIR of entries, ~8 us per feature: profiles/r02_sae_notes.md.)
+    // of three dependent L2 round trips PER PAIR of entries.)
     int my_b = 0;
     float my_a = 0.f, my_dp = 0.f;
     {
@@ -554,7 +554,7 @@ __global__ void __launch_bounds__(256) k_sae_grads(const int* __restrict__ off, 
   }
   // the -b_dec path, sum_f gb_enc[f] W_encT[f]: per-lane register partials over this warp's features, one shared-memory
   // reduction per CTA (the per-feature shared atomics of the first version cost 24 x 64 cycles of the LSU per feature -- the
-  // whole kernel ran at the ATOMS rate, profiles/r02_sae_notes.md)
+  // whole kernel ran at the ATOMS rate)
 #pragma unroll
   for (int i = 0; i < CHUNKS; ++i) {
     const int c4 = i * 32 + lane;
@@ -668,10 +668,11 @@ __global__ void __launch_bounds__(256) k_sae_grads_long(const int* __restrict__ 
 // 5c. squared norm of the completed hot-feature rows (not additive over chunks, so it waits for 5b)
 __global__ void __launch_bounds__(256) k_sae_norm_long(const float* __restrict__ gW_dec, const float* __restrict__ gW_encT,
                                                        const float* __restrict__ gb_enc, SaeScalars* __restrict__ sc, int d,
-                                                       const SaeWorkHeader* __restrict__ work, const int* __restrict__ work_feats) {
+                                                       const SaeWorkHeader* work, const int* __restrict__ work_feats) {
   pb_pdl();
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  const int n = work->n_long;
+  // written by k_sae_grads two launches back: a read-only (__restrict__ const) load of it was scheduled above griddepcontrol.wait
+  const int n = *reinterpret_cast<const volatile int*>(&work->n_long);
   float nsq = 0.f;
   for (int li = blockIdx.x * nw + warp; li < n; li += gridDim.x * nw) {
     const int f = work_feats[li];
@@ -726,7 +727,7 @@ struct AdamHyper { float lr, beta1, beta2, eps, bc1, bc2_sqrt; };  // bc1 = 1-be
 // torch.optim.Adam (single tensor, no amsgrad / weight decay): m, v exactly as torch computes them; the parameter update
 // -(lr / bc1) m / (sqrt(v) / bc2_sqrt + eps) uses MUFU sqrt / reciprocal approximations (relative error ~1e-7 of an update that is
 // itself ~lr relative to the parameter: 1e-10 on the parameter, against a 1e-4 parity bar).  The IEEE sqrt + two divisions of the
-// first version were ~30 of the ~45 instructions per element and made the optimizer issue-bound (profiles/r02_sae_notes.md).
+// first version were ~30 of the ~45 instructions per element and made the optimizer issue-bound.
 __device__ __forceinline__ float adam_update(float p, float gr, float& m, float& v, const AdamHyper& h) {
   m = h.beta1 * m + (1.f - h.beta1) * gr;
   v = h.beta2 * v + (1.f - h.beta2) * gr * gr;

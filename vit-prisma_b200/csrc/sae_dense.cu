@@ -1,7 +1,7 @@
 // sae_dense.cu -- the pieces of the SAE training step that are dense in d_sae:
 //   * activation_fn_str = "relu" (+ L1 sparsity term), the reference's default activation (sae/sae.py:617-626, 810-839):
 //     feature_acts, the decoder product and all four weight gradients are dense [tokens, d_sae] / [d_sae, d_in] GEMMs; they
-//     run on pb_gemm (tcgen05, 3xTF32) and the kernels here are the glue between them -- transposes (pb_gemm takes K-major
+//     run on pb_gemm (wgmma, 3xTF32) and the kernels here are the glue between them -- transposes (pb_gemm takes K-major
 //     operands), statistics, loss / dL/d(out), the ReLU + L1 backward mask, bias gradients, the global gradient norm;
 //   * the ghost-grad auxiliary loss on dead features (sae/sae.py:151-179; train_sae.py:330-332), for either activation:
 //     column gather exp(hidden_pre[:, dead]), the per-row residual / rescale / loss / dL/dG kernel, row gathers and

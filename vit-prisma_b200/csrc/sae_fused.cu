@@ -1,14 +1,14 @@
-// sae_fused.cu -- fused SAE encoder -> TopK for sm_100a: the dense pre-activation matrix hidden_pre [tokens, d_sae] is never
+// sae_fused.cu -- fused SAE encoder -> TopK for sm_90a: the dense pre-activation matrix hidden_pre [tokens, d_sae] is never
 // written to HBM (reference sae/sae.py:557-581 `sae_in @ W_enc + b_enc` followed by TopK.forward :795-808 `torch.topk`).
 //
 // Approximate-then-rescore, exact by construction:
-//   1. k_enc_cand     persistent tcgen05 GEMM, ONE kind::tf32 pass (the fp32 operands are read by the tensor core with their 13
-//                     low mantissa bits ignored), 128 x 256 tiles, accumulators double-buffered in TMEM.  The epilogue never
-//                     stores the tile: every thread owns one token row x 128 feature columns of it (TMEM's native layout) and
-//                     keeps that segment's C_KEEP largest values as packed keys (order-preserving int of the value, the low
-//                     7 bits replaced by the column inside the segment) with a branch-free insertion network, then writes
-//                     C_KEEP x 4 bytes.  Per token: d_sae / 128 segments x C_KEEP keys (6 KB at d_sae = 24576) instead of a
-//                     98 KB dense row.
+//   1. k_enc_cand     persistent wgmma GEMM, ONE tf32 pass (the fp32 operands are read by the tensor core with their 13 low
+//                     mantissa bits ignored), 128 x 128 tiles: a tile's columns are one 128-feature segment.  The epilogue never
+//                     stores the tile: every thread keeps the C_KEEP largest of the 32 values it holds of each of its two token
+//                     rows as packed keys (order-preserving int of the value, the low 7 bits replaced by the column inside the
+//                     segment) with a branch-free insertion network, the four threads sharing a row merge their lists by
+//                     shuffles, and one of them writes C_KEEP x 4 bytes.  Per token: d_sae / 128 segments x C_KEEP keys (6 KB at
+//                     d_sae = 24576) instead of a 98 KB dense row.
 //   2. k_cand_select  one CTA per token: the m_cand best keys of the row (threshold from per-thread bests, rank by counting),
 //                     EXACT fp32 re-evaluation of those m_cand pre-activations (FFMA dot products against W_encT rows),
 //                     exact top-k of the re-scored values (ties -> lower index, sorted descending), and a proof that no
@@ -32,71 +32,25 @@ __device__ __forceinline__ int f2ord(float v) {           // monotone float -> s
 __device__ __forceinline__ float ord2f(int k) { return __int_as_float(k ^ ((k >> 31) & 0x7fffffff)); }
 __device__ __forceinline__ bool key_gt_f(float va, int ia, float vb, int ib) { return va > vb || (va == vb && ia < ib); }
 
-#ifndef PB_ENC_PAIR_DEFAULT
-#define PB_ENC_PAIR_DEFAULT 0      // flipped to 1 once measured faster on the B200 (profiles/r02_sae_notes.md)
-#endif
-constexpr int FZ_BN = 256;       // tile columns
-constexpr int FZ_STAGES = 4;     // 4 x (16 KB A + 32 KB B) = 192 KB operand ring
-constexpr int FZ_NEPI = 8;       // epilogue warps: 4 TMEM lane quarters x 2 column halves
-constexpr int FZ_SEG = 128;      // columns per thread segment (= FZ_BN / 2)
-constexpr int FZ_THREADS = 64 + FZ_NEPI * 32;
-using FzCfg = TcCfg<float, 1, FZ_BN, FZ_STAGES>;
+constexpr int FZ_SEG = 128;      // columns per segment = tile columns (TC_BN)
+constexpr int FZ_STAGES = 6;     // 6 x (16 KB A + 16 KB B) = 192 KB operand ring
+using FzCfg = TcCfg<float, 1, FZ_STAGES>;
 constexpr int FZ_SMEM = FzCfg::RING_BYTES + 1024 + 256;
+static_assert(FZ_SEG == TC_BN, "a tile is one segment");
 
-// One epilogue warp's share of one finished accumulator: thread = one token row x one 128-feature segment; keeps the segment's
-// C_KEEP largest pre-activations as packed keys and writes them.  `release` is called once the accumulator has been read.
-template <int C_KEEP, typename Release>
-__device__ __forceinline__ void enc_cand_epilogue(uint32_t tmem_base, int ab, int quarter, int cbase, int lane, int m0, int n0, int M, int N,
-                                                  const float* __restrict__ bias, int* __restrict__ cand, Release release) {
-  const int nseg = N / FZ_SEG;
-  const int row = m0 + quarter * 32 + lane;
-  const bool seg_in = (n0 + cbase) < N;          // N % 128 == 0: a segment is entirely inside or outside the matrix
-  int s[C_KEEP];
+__device__ __forceinline__ void key_insert(int (&s)[8], int x, int n) {   // s[0, n) stays sorted descending
 #pragma unroll
-  for (int i = 0; i < C_KEEP; ++i) s[i] = INT_MIN;
-#pragma unroll 1
-  for (int c = 0; c < FZ_SEG / 32; ++c) {
-    uint32_t r[32];
-    tmem_ld32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(ab * FZ_BN + cbase + c * 32), r);
-    tmem_ld_wait();
-    if (c == FZ_SEG / 32 - 1) {                  // last read of this accumulator: hand it back to the MMA warp
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) release();
-    }
-    if (seg_in) {
-      const float* bp = bias + n0 + cbase + c * 32;
-#pragma unroll
-      for (int q = 0; q < 8; ++q) {
-        float bb[4];
-        ld4(bp + 4 * q, bb);                     // same address in every lane: one broadcast transaction
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          int x = (f2ord(__uint_as_float(r[4 * q + j]) + bb[j]) & ~127) | (c * 32 + 4 * q + j);
-#pragma unroll
-          for (int i = 0; i < C_KEEP; ++i) {     // insertion network: s[] stays sorted descending
-            const int hi = max(s[i], x);
-            x = min(s[i], x);
-            s[i] = hi;
-          }
-        }
-      }
-    }
-  }
-  if (seg_in && row < M) {
-    int* dst = cand + ((int64_t)row * nseg + (n0 + cbase) / FZ_SEG) * C_KEEP;
-    if (C_KEEP % 4 == 0) {
-#pragma unroll
-      for (int i = 0; i < C_KEEP / 4; ++i) reinterpret_cast<int4*>(dst)[i] = make_int4(s[4 * i], s[4 * i + 1], s[4 * i + 2], s[4 * i + 3]);
-    } else {
-#pragma unroll
-      for (int i = 0; i < C_KEEP / 2; ++i) reinterpret_cast<int2*>(dst)[i] = make_int2(s[2 * i], s[2 * i + 1]);
+  for (int i = 0; i < 8; ++i) {
+    if (i < n) {
+      const int hi = max(s[i], x);
+      x = min(s[i], x);
+      s[i] = hi;
     }
   }
 }
 
 template <int C_KEEP>
-__global__ void __launch_bounds__(FZ_THREADS, 1)
+__global__ void __launch_bounds__(TC_THREADS, 1)
 k_enc_cand(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, int K, int M, int N,
            const float* __restrict__ bias, int* __restrict__ cand, int num_m_tiles, int num_n_tiles) {
   using C = FzCfg;
@@ -107,46 +61,37 @@ k_enc_cand(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
   const uint32_t bar_base = ring + C::RING_BYTES;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (FZ_STAGES + s); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * FZ_STAGES + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * FZ_STAGES + 2 + a); };
-  const uint32_t tmem_ptr_addr = bar_base + 8u * (2 * FZ_STAGES + 4);
-  volatile uint32_t* tmem_ptr_generic = reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_ptr_addr - smem0));
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = warp >> 2;
   const int num_kb = (K + C::BK - 1) / C::BK;
   const int num_tiles = num_m_tiles * num_n_tiles;
-  // m-fastest raster: the CTAs in flight share one 256-feature slab of the dictionary and walk the token tiles, so W_encT
+  const int nseg = N / FZ_SEG;
+  // m-fastest raster: the CTAs in flight share one 128-feature slab of the dictionary and walk the token tiles, so W_encT
   // (75 MB at d_sae = 24576) streams from HBM once while sae_in (12.6 MB) stays L2-resident.
   auto tile_m = [&](int tile) { return tile % num_m_tiles; };
   auto tile_n = [&](int tile) { return tile / num_m_tiles; };
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB);
-    for (int s = 0; s < FZ_STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(tfull_bar(a), 1); mbar_init(tempty_bar(a), FZ_NEPI); }
+    for (int s = 0; s < FZ_STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 2); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_ptr_addr), "r"((uint32_t)(2 * FZ_BN)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_generic;
-  pb_pdl_wait();            // barriers initialised, TMEM allocated, tensor maps prefetched: now the prep kernel's sae_in must be complete
+  pb_pdl_wait();            // barriers initialised, tensor maps prefetched: now the prep kernel's sae_in must be complete
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ===================== TMA producer =====================
-    if (lane == 0) {
+    reg_dealloc<40>();
+    if (threadIdx.x == 0) {
       uint32_t it = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int m0 = tile_m(tile) * TC_BM, n0 = tile_n(tile) * FZ_BN;
+        const int m0 = tile_m(tile) * TC_BM, n0 = tile_n(tile) * TC_BN;
         for (int kb = 0; kb < num_kb; ++kb, ++it) {
           const int s = it % FZ_STAGES;
           const uint32_t ph = (it / FZ_STAGES) & 1;
-          mbar_wait(empty_bar(s), ph ^ 1);
+          mbar_wait<false>(empty_bar(s), ph ^ 1);
           mbar_expect_tx(full_bar(s), C::STAGE_BYTES);
           const uint32_t sa = ring + s * C::STAGE_BYTES;
           tma_load_2d(sa, &tmA, full_bar(s), kb * C::BK, m0);
@@ -154,174 +99,73 @@ k_enc_cand(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer: one kind::tf32 pass =====================
-    if (lane == 0) {
-      uint32_t it = 0;
-      int li = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++li) {
-        const int ab = li & 1;
-        const uint32_t aph = (li >> 1) & 1;
-        mbar_wait(tempty_bar(ab), aph ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(ab * FZ_BN);
-        for (int kb = 0; kb < num_kb; ++kb, ++it) {
-          const int s = it % FZ_STAGES;
-          const uint32_t ph = (it / FZ_STAGES) & 1;
-          mbar_wait(full_bar(s), ph);
-          tc_fence_after();
-          const uint32_t sa = ring + s * C::STAGE_BYTES;
-          const uint32_t sb = sa + C::A_BYTES;
+    return;
+  }
+  // ===================== consumers: one tf32 pass, then per-row top-C_KEEP of the segment as packed keys =====================
+  reg_alloc<232>();
+  const int c = wg - 1, wq = warp & 3, tid = threadIdx.x & 127;
+  float acc[64];
+  uint32_t it = 0;
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    const int m0 = tile_m(tile) * TC_BM, n0 = tile_n(tile) * TC_BN;
+    int prev_s = -1;
+    for (int kb = 0; kb < num_kb; ++kb, ++it) {
+      const int s = it % FZ_STAGES;
+      const uint32_t ph = (it / FZ_STAGES) & 1;
+      mbar_wait<false>(full_bar(s), ph);
+      const uint32_t sa = ring + s * C::STAGE_BYTES + c * 64 * 128;
+      const uint32_t sb = ring + s * C::STAGE_BYTES + C::A_BYTES;
+      wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < 128 / C::UMMA_K_BYTES; ++k) {
-            const uint32_t koff = k * C::UMMA_K_BYTES;
-            tc_mma<1>(d_tmem, make_smem_desc(sa + koff), make_smem_desc(sb + koff), C::IDESC, (kb | k) != 0 ? 1u : 0u);
+      for (int k = 0; k < C::KSTEPS; ++k) wgmma_tf32_n128(acc, make_smem_desc(sa + 32 * k), make_smem_desc(sb + 32 * k), (kb | k) != 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (prev_s >= 0 && tid == 0) mbar_arrive(empty_bar(prev_s));
+      prev_s = s;
+    }
+    wgmma_wait<0>();
+    wgmma_fence_acc(acc);
+    if (tid == 0) mbar_arrive(empty_bar(prev_s));
+
+    // accumulator element i of this thread: row 16 wq + lane / 4 + 8 ((i >> 1) & 1), column 8 (i >> 2) + 2 (lane % 4) + (i & 1)
+    int s0[8], s1[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) { s0[i] = INT_MIN; s1[i] = INT_MIN; }
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const int col = 8 * j + 2 * (lane & 3);
+      const float2 bb = *reinterpret_cast<const float2*>(bias + n0 + col);
+      key_insert(s0, (f2ord(acc[4 * j] + bb.x) & ~127) | col, C_KEEP);
+      key_insert(s0, (f2ord(acc[4 * j + 1] + bb.y) & ~127) | (col + 1), C_KEEP);
+      key_insert(s1, (f2ord(acc[4 * j + 2] + bb.x) & ~127) | col, C_KEEP);
+      key_insert(s1, (f2ord(acc[4 * j + 3] + bb.y) & ~127) | (col + 1), C_KEEP);
+    }
+    // the four lanes of a quad hold disjoint columns of the same two rows: merge their lists (keys are distinct)
+#pragma unroll
+    for (int off = 1; off <= 2; off <<= 1) {
+      int t0[8], t1[8];
+#pragma unroll
+      for (int i = 0; i < C_KEEP; ++i) { t0[i] = __shfl_xor_sync(0xffffffffu, s0[i], off); t1[i] = __shfl_xor_sync(0xffffffffu, s1[i], off); }
+#pragma unroll
+      for (int i = 0; i < C_KEEP; ++i) { key_insert(s0, t0[i], C_KEEP); key_insert(s1, t1[i], C_KEEP); }
+    }
+    if ((lane & 3) == 0) {
+      const int row = m0 + 64 * c + 16 * wq + (lane >> 2);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int* sv = h == 0 ? s0 : s1;
+        if (row + 8 * h < M) {
+          int* dst = cand + ((int64_t)(row + 8 * h) * nseg + n0 / FZ_SEG) * C_KEEP;
+          if (C_KEEP % 4 == 0) {
+#pragma unroll
+            for (int i = 0; i < C_KEEP / 4; ++i) reinterpret_cast<int4*>(dst)[i] = make_int4(sv[4 * i], sv[4 * i + 1], sv[4 * i + 2], sv[4 * i + 3]);
+          } else {
+#pragma unroll
+            for (int i = 0; i < C_KEEP / 2; ++i) reinterpret_cast<int2*>(dst)[i] = make_int2(sv[2 * i], sv[2 * i + 1]);
           }
-          tc_commit(empty_bar(s));
-        }
-        tc_commit(tfull_bar(ab));
-      }
-    }
-  } else {
-    // ===================== epilogue: per-row, per-128-column top-C_KEEP as packed keys =====================
-    const int e = warp - 2;
-    const int quarter = warp & 3;          // TMEM lane quarter this warp may read
-    const int cbase = (e >> 2) * FZ_SEG;   // column half of the tile
-    int li = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++li) {
-      const int m0 = tile_m(tile) * TC_BM, n0 = tile_n(tile) * FZ_BN;
-      const int ab = li & 1;
-      const uint32_t aph = (li >> 1) & 1;
-      mbar_wait(tfull_bar(ab), aph);
-      tc_fence_after();
-      enc_cand_epilogue<C_KEEP>(tmem_base, ab, quarter, cbase, lane, m0, n0, M, N, bias, cand, [&] { mbar_arrive(tempty_bar(ab)); });
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)(2 * FZ_BN)) : "memory");
-  }
-}
-
-
-// ---------------------------------------------------------------------------------------------------------------------
-// CTA-pair variant (tcgen05 cta_group::2, protocol of gemm_tc_pair.cuh): the two CTAs of a cluster compute a 256-token x 256-feature
-// tile with one MMA stream issued by the leader; each CTA loads its own 128 token rows and HALF of the dictionary tile, so the
-// per-SM operand ingest drops from 48 KB to 32 KB per k-block (the one-CTA kernel runs the tensor pipe at 76 % of its active cycles
-// because its 67 B/clk/SM operand demand exceeds what TMA delivers, profiles/r02_sae_notes.md).  Six 32 KB stages.
-constexpr int FZP_STAGES = 6;
-constexpr int FZP_A_BYTES = TC_BM * 128, FZP_BH_BYTES = (FZ_BN / 2) * 128, FZP_STAGE_BYTES = FZP_A_BYTES + FZP_BH_BYTES;
-constexpr int FZP_SMEM = FZP_STAGES * FZP_STAGE_BYTES + 1024 + 256;
-constexpr uint32_t FZP_IDESC = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(FZ_BN >> 3) << 17) | ((uint32_t)(256 >> 4) << 24);   // tf32, M = 256 across the pair
-
-template <int C_KEEP>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(FZ_THREADS, 1)
-k_enc_cand_pair(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmBh, int K, int M, int N,
-                const float* __restrict__ bias, int* __restrict__ cand, int num_m_tiles /* of 256 rows */, int num_n_tiles) {
-  pb_pdl_trigger();
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem0 = smem_u32(smem_raw);
-  const uint32_t ring = (smem0 + 1023u) & ~1023u;
-  const uint32_t bar_base = ring + FZP_STAGES * FZP_STAGE_BYTES;
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };                            // used in the leader only
-  auto empty_bar = [&](int s) { return bar_base + 8u * (FZP_STAGES + s); };            // one per CTA
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * FZP_STAGES + a); };        // one per CTA
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * FZP_STAGES + 2 + a); };   // used in the leader only
-  const uint32_t tmem_ptr_addr = bar_base + 8u * (2 * FZP_STAGES + 4);
-  volatile uint32_t* tmem_ptr_generic = reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_ptr_addr - smem0));
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int cluster_id = blockIdx.x >> 1, n_clusters = gridDim.x >> 1;
-  constexpr int BK = 32;
-  const int num_kb = (K + BK - 1) / BK;
-  const int num_tiles = num_m_tiles * num_n_tiles;
-  auto tile_m = [&](int tile) { return tile % num_m_tiles; };        // m-fastest raster, as in k_enc_cand
-  auto tile_n = [&](int tile) { return tile / num_m_tiles; };
-
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&tmA);
-    prefetch_tmap(&tmBh);
-    for (int s = 0; s < FZP_STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(tfull_bar(a), 1); mbar_init(tempty_bar(a), 2 * FZ_NEPI); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_ptr_addr), "r"((uint32_t)(2 * FZ_BN)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();                                        // peer barriers initialised before anyone signals them
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_generic;
-  pb_pdl_wait();
-
-  if (warp == 0) {
-    if (lane == 0) {                                         // TMA producer (both CTAs)
-      uint32_t it = 0;
-      for (int tile = cluster_id; tile < num_tiles; tile += n_clusters) {
-        const int m0 = tile_m(tile) * 256 + (int)rank * TC_BM;
-        const int n0 = tile_n(tile) * FZ_BN + (int)rank * (FZ_BN / 2);
-        for (int kb = 0; kb < num_kb; ++kb, ++it) {
-          const int s = it % FZP_STAGES;
-          const uint32_t ph = (it / FZP_STAGES) & 1;
-          mbar_wait(empty_bar(s), ph ^ 1);
-          if (leader) mbar_expect_tx(full_bar(s), 2u * FZP_STAGE_BYTES);   // bytes of BOTH CTAs land on the leader's barrier
-          const uint32_t sa = ring + s * FZP_STAGE_BYTES;
-          tma_load_2d_pair(sa, &tmA, full_bar(s), kb * BK, m0);
-          tma_load_2d_pair(sa + FZP_A_BYTES, &tmBh, full_bar(s), kb * BK, n0);
         }
       }
     }
-  } else if (warp == 1) {
-    if (leader && lane == 0) {                               // MMA issuer (leader only): one kind::tf32 pass
-      uint32_t it = 0;
-      int li = 0;
-      for (int tile = cluster_id; tile < num_tiles; tile += n_clusters, ++li) {
-        const int ab = li & 1;
-        const uint32_t aph = (li >> 1) & 1;
-        mbar_wait(tempty_bar(ab), aph ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(ab * FZ_BN);
-        for (int kb = 0; kb < num_kb; ++kb, ++it) {
-          const int s = it % FZP_STAGES;
-          const uint32_t ph = (it / FZP_STAGES) & 1;
-          mbar_wait(full_bar(s), ph);
-          tc_fence_after();
-          const uint32_t sa = ring + s * FZP_STAGE_BYTES;
-          const uint32_t sb = sa + FZP_A_BYTES;
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            tc_mma_pair<1>(d_tmem, make_smem_desc(sa + 32 * k), make_smem_desc(sb + 32 * k), FZP_IDESC, (kb | k) != 0 ? 1u : 0u);
-          tc_commit_pair(empty_bar(s));
-        }
-        tc_commit_pair(tfull_bar(ab));
-      }
-    }
-  } else {
-    const int e = warp - 2;
-    const int quarter = warp & 3;
-    const int cbase = (e >> 2) * FZ_SEG;
-    int li = 0;
-    for (int tile = cluster_id; tile < num_tiles; tile += n_clusters, ++li) {
-      const int m0 = tile_m(tile) * 256 + (int)rank * TC_BM, n0 = tile_n(tile) * FZ_BN;
-      const int ab = li & 1;
-      const uint32_t aph = (li >> 1) & 1;
-      mbar_wait(tfull_bar(ab), aph);
-      tc_fence_after();
-      enc_cand_epilogue<C_KEEP>(tmem_base, ab, quarter, cbase, lane, m0, n0, M, N, bias, cand, [&] { mbar_arrive_remote(tempty_bar(ab), 0); });
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();                                        // the peer may still be reading its half of TMEM / our shared memory
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)(2 * FZ_BN)) : "memory");
   }
 }
 
@@ -365,8 +209,7 @@ __device__ __forceinline__ int sel_pos(unsigned long long it) { return (int)(0xF
 //   3. rounds: exactly re-score the first m_cur sorted candidates (m_cand, then +16 per round), take the exact top-k of those,
 //      and try to prove no other feature can beat the k-th:   ub(best key not yet re-scored) + E_row < tau_k.  Most rows are
 //      proven in the first round; a row that runs out of sorted candidates (or whose segment kept-lists saturate) is listed.
-// (The first version ranked by counting -- 256^2 + G^2 shared-memory compares per row -- and was ALU-bound at 205 us per launch,
-//  75 % issue-active, with the re-scoring gathers a small part of it: profiles/r02_sae_notes.md.)
+// (A first version ranked by counting -- 256^2 + G^2 shared-memory compares per row -- and was ALU-bound.)
 template <int SPT>
 __global__ void __launch_bounds__(256) k_cand_select(const int* __restrict__ cand, int nseg, int c_keep, const float* __restrict__ sae_in,
                                                      const float* __restrict__ W_encT, const float* __restrict__ b_enc,
@@ -548,7 +391,11 @@ __global__ void __launch_bounds__(256) k_cand_select(const int* __restrict__ can
       const int u = max(u_rest, sat_key);
       const float u_val = u == INT_MIN ? -INFINITY : ord2f((u & ~127) | 127);               // upper end of the key's value bucket
       // |tf32 product - exact| = |a_lo.w + a_hi.w_lo| <= ||a_lo|| max||w|| + ||a|| max||w_lo||   (Cauchy-Schwarz, per row)
-      const float E = err_scale * (a_lo_norm * wnorm_max[0] + a_norm * wnorm_max[1]) + fabsf(tau_exact) * 1.2207031e-4f;
+      // + the fp32 accumulation of the wgmma chain: ceil(d / 8) k-steps, each allowed 4 units of 2^-23 of the magnitudes entering it
+      //   (accumulator and eight products: a step that truncates instead of rounding costs 2, the rest is margin), every one of
+      //   them bounded by sum_i |a_i w_i| <= ||a|| max||w||
+      const float acc_err = (float)((d + 7) / 8) * 4.76837158e-7f * a_norm * wnorm_max[0];
+      const float E = err_scale * (a_lo_norm * wnorm_max[0] + a_norm * wnorm_max[1]) + acc_err + fabsf(tau_exact) * 1.2207031e-4f;
       ok = !overflow && m_cur >= k && (u_val + E < tau_exact);
     }
     if (ok || m_cur >= Gs) break;
@@ -662,47 +509,21 @@ __global__ void __launch_bounds__(256) k_rownorm_max(const float* __restrict__ W
   }
 }
 
-// PB_ENC_PAIR=0 forces the one-CTA kernel, =1 the CTA-pair kernel (default: pairs when at least two 256-token tiles exist)
-static int enc_pair_mode() {
-  const char* v = getenv("PB_ENC_PAIR");       // read per call: tests flip it inside one process
-  return v && *v ? atoi(v) : -1;
-}
-
-template <int C_KEEP>
-int launch_enc_cand_pair(const PbSaeEncode* e, cudaStream_t st) {
-  CUtensorMap tmA, tmBh;
-  PB_TRY(make_map(&tmA, e->sae_in, PB_F32, e->rows, e->d, e->d, TC_BM));
-  PB_TRY(make_map(&tmBh, e->W_encT, PB_F32, e->F, e->d, e->d, FZ_BN / 2));       // box = this CTA's half of the dictionary tile
-  auto kern = k_enc_cand_pair<C_KEEP>;
-  static bool attr_done = false;
-  if (!attr_done) {
-    PB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, FZP_SMEM));
-    attr_done = true;
-  }
-  const int num_m = (e->rows + 255) / 256, num_n = (e->F + FZ_BN - 1) / FZ_BN;
-  int clusters = pb_sm_count() / 2;
-  if (clusters > num_m * num_n) clusters = num_m * num_n;
-  PB_LAUNCH_PDL(kern, 2 * clusters, FZ_THREADS, FZP_SMEM, st, tmA, tmBh, e->d, e->rows, e->F, e->b_enc, e->cand, num_m, num_n);
-  return PB_OK;
-}
-
 template <int C_KEEP>
 int launch_enc_cand(const PbSaeEncode* e, cudaStream_t st) {
-  const int pm = enc_pair_mode();
-  if (pm == 1 || (pm < 0 && PB_ENC_PAIR_DEFAULT && e->rows >= 512)) return launch_enc_cand_pair<C_KEEP>(e, st);
   CUtensorMap tmA, tmB;
   PB_TRY(make_map(&tmA, e->sae_in, PB_F32, e->rows, e->d, e->d, TC_BM));
-  PB_TRY(make_map(&tmB, e->W_encT, PB_F32, e->F, e->d, e->d, FZ_BN));
+  PB_TRY(make_map(&tmB, e->W_encT, PB_F32, e->F, e->d, e->d, TC_BN));
   auto kern = k_enc_cand<C_KEEP>;
   static bool attr_done = false;
   if (!attr_done) {
     PB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, FZ_SMEM));
     attr_done = true;
   }
-  const int num_m = (e->rows + TC_BM - 1) / TC_BM, num_n = (e->F + FZ_BN - 1) / FZ_BN;
+  const int num_m = (e->rows + TC_BM - 1) / TC_BM, num_n = (e->F + TC_BN - 1) / TC_BN;
   int grid = pb_sm_count();
   if (grid > num_m * num_n) grid = num_m * num_n;
-  PB_LAUNCH_PDL(kern, grid, FZ_THREADS, FZ_SMEM, st, tmA, tmB, e->d, e->rows, e->F, e->b_enc, e->cand, num_m, num_n);
+  PB_LAUNCH_PDL(kern, grid, TC_THREADS, FZ_SMEM, st, tmA, tmB, e->d, e->rows, e->F, e->b_enc, e->cand, num_m, num_n);
   return PB_OK;
 }
 

@@ -1,5 +1,5 @@
-// tc_common.cuh -- tcgen05 / TMEM / TMA / mbarrier PTX wrappers, tile configuration and tensor-map construction shared by
-// the tensor-core kernels of this library (gemm_tc.cu, sae_fused.cu).  sm_100a only.
+// tc_common.cuh -- wgmma / TMA / mbarrier PTX wrappers, tile configuration and tensor-map construction shared by the
+// tensor-core kernels of this library (gemm_tc.cu, sae_fused.cu).  sm_90a only.
 #pragma once
 #include "common.cuh"
 #include <cuda.h>
@@ -16,7 +16,10 @@ __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
-// Bounded wait: a protocol bug turns into a trap (-> CUDA error) instead of a hung GPU.
+// Bounded wait: a protocol bug turns into a trap (-> CUDA error) instead of a hung GPU.  REPORT prints which block / thread /
+// barrier / parity timed out.  Kernels that issue wgmma pass REPORT = false in every wait: a printf (a function call) anywhere in
+// such a kernel, even on a branch no wgmma is in flight on, makes ptxas serialise all of its wgmma instructions (warning C7510).
+template <bool REPORT = true>
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   const long long t0 = clock64();
   for (;;) {
@@ -29,8 +32,9 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
         : "r"(bar), "r"(parity)
         : "memory");
     if (done) return;
-    if (clock64() - t0 > 4000000000LL) {  // ~2 s at 2 GHz
-      printf("gemm_tc: mbarrier wait timed out (block %d,%d thread %d bar %u parity %u)\n", blockIdx.x, blockIdx.y, threadIdx.x, bar, parity);
+    if (clock64() - t0 > 4000000000LL) {   // ~2 s at 2 GHz
+      if (REPORT)
+        printf("prisma: mbarrier wait timed out (block %d thread %d bar 0x%x parity %u)\n", blockIdx.x, threadIdx.x, bar, parity);
       __trap();
     }
   }
@@ -43,72 +47,73 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+// ---- wgmma (warpgroup MMA, sm_90a): both operands K-major in shared memory, fp32 accumulators in registers
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// the accumulators are handed to the asm as operands; this keeps later reads of them behind the wait
+__device__ __forceinline__ void wgmma_fence_acc(float (&d)[64]) {
+#pragma unroll
+  for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-template <int KIND>  // 0: kind::f16 (bf16 in), 1: kind::tf32
-__device__ __forceinline__ void tc_mma(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  if (KIND == 0) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  } else {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  }
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
+// the 64 fp32 accumulator operands of an m64n128 wgmma: asm operand list and constraints (d is the float[64] array)
+#define PB_ACC64_REGS "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+#define PB_ACC64_OUT "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+// D[64 x 128] (+)= A[64 x K-step] * B[128 x K-step]^T; accumulate = 0 overwrites D.  One K-step is 32 bytes of each row.
+__device__ __forceinline__ void wgmma_tf32_n128(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+      "{" PB_ACC64_REGS "}, "
+      "%64, %65, p, 1, 1;\n\t}"
+      : PB_ACC64_OUT
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_bf16_n128(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{" PB_ACC64_REGS "}, "
+      "%64, %65, p, 1, 1, 0, 0;\n\t}"
+      : PB_ACC64_OUT
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
 
-// Shared-memory matrix descriptor, K-major operand, 128-byte swizzle (cute::UMMA::SmemDescriptor):
+// named barrier over the 128 threads of one warpgroup (ids 1.. : 0 is __syncthreads)
+// register budget per warpgroup (warpgroup-wide): the producer keeps 40, the two consumers take 232 each (64 accumulators + epilogue)
+template <int N> __device__ __forceinline__ void reg_dealloc() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N> __device__ __forceinline__ void reg_alloc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+__device__ __forceinline__ void wg_sync(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+
+// Shared-memory matrix descriptor (sm_90 GMMA), K-major operand, 128-byte swizzle:
 //   [0,14)  start address >> 4        [16,30) leading byte offset >> 4 (unused for swizzled K-major: 1)
 //   [32,46) stride byte offset >> 4   = 1024 B between 8-row groups (rows are 128 B, stored densely by TMA)
-//   [46,48) descriptor version = 1 (sm_100)      [61,64) layout type = 2 (SWIZZLE_128B)
+//   [62,64) layout type = 1 (SWIZZLE_128B).  Tiles are 1024-byte aligned, so the base offset [49,52) is 0.
+// The K-steps inside a 128-byte row advance the start address by 32 bytes (the swizzle is a function of the address).
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
   d |= (uint64_t)1 << 16;
   d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
 }
 
-constexpr int TC_BM = 128;
-constexpr int TC_THREADS = 192;
+constexpr int TC_BM = 128;           // tile rows: two consumer warpgroups of 64 rows each
+constexpr int TC_BN = 128;           // tile columns: one m64n128 accumulator (64 registers) per consumer thread
+constexpr int TC_THREADS = 384;      // warpgroup 0: TMA producer; warpgroups 1, 2: wgmma + epilogue
 
-template <typename T, int NPASS, int BN, int STAGES>
+template <typename T, int NPASS, int STAGES>
 struct TcCfg {
   static constexpr int ES = sizeof(T);
   static constexpr int BK = 128 / ES;       // elements per 128-byte k-slab
-  static constexpr int UMMA_K_BYTES = 32;   // one tcgen05.mma consumes 32 bytes of K per row
+  static constexpr int KSTEPS = 4;          // one wgmma consumes 32 bytes of K per row
   static constexpr int A_BYTES = TC_BM * 128;
-  static constexpr int B_BYTES = BN * 128;
+  static constexpr int B_BYTES = TC_BN * 128;
   static constexpr int NOP = NPASS == 3 ? 2 : 1;  // operand copies per matrix (hi [+ lo])
   static constexpr int STAGE_BYTES = NOP * (A_BYTES + B_BYTES);
   static constexpr int RING_BYTES = STAGES * STAGE_BYTES;
-  static constexpr int SMEM_BYTES = RING_BYTES + 1024 /*alignment slack*/ + 256 /*barriers + tmem ptr*/;
-  static constexpr uint32_t FMT = sizeof(T) == 2 ? 1u : 2u;  // F16F32Format: BF16 = 1, TF32 = 2
-  // cute::UMMA::InstrDescriptor: c_format F32 [4,6) | a_format [7,10) | b_format [10,13) | a/b K-major (0) | N>>3 [17,23) | M>>4 [24,29)
-  static constexpr uint32_t IDESC = (1u << 4) | (FMT << 7) | (FMT << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(TC_BM >> 4) << 24);
 };
 
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
@@ -147,57 +152,6 @@ int make_map(CUtensorMap* map, const void* ptr, int dtype, int64_t rows, int64_t
     return PB_ECUDA;
   }
   return PB_OK;
-}
-
-// ---------------------------------------------------------------------------------------------------------------------
-// CTA pairs (tcgen05 cta_group::2): shared by gemm_tc_pair.cuh and the fused SAE encoder (sae_fused.cu)
-constexpr uint32_t PEER_BIT_MASK = 0xFEFFFFFFu;            // shared::cluster address of the same offset in CTA rank 0 of the pair
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.aligned;\n\tbarrier.cluster.wait.aligned;" ::: "memory");
-}
-// TMA load whose complete_tx lands on the LEADER's barrier (both CTAs execute it)
-__device__ __forceinline__ void tma_load_2d_pair(uint32_t dst, const CUtensorMap* map, uint32_t leader_bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(dst),
-      "l"(reinterpret_cast<uint64_t>(map)), "r"(leader_bar & PEER_BIT_MASK), "r"(c0), "r"(c1)
-      : "memory");
-}
-template <int KIND>
-__device__ __forceinline__ void tc_mma_pair(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  if (KIND == 0) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  } else {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  }
-}
-// arrive::one on the barrier at this offset in BOTH CTAs once the MMAs issued so far have completed
-__device__ __forceinline__ void tc_commit_pair(uint32_t bar) {
-  const uint16_t mask = 0x3;
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar), "h"(mask)
-               : "memory");
-}
-// arrive on the barrier at this offset in CTA `rank` of the cluster
-__device__ __forceinline__ void mbar_arrive_remote(uint32_t bar, uint32_t rank) {
-  asm volatile(
-      "{\n\t.reg .b32 remote;\n\t"
-      "mapa.shared::cluster.u32 remote, %0, %1;\n\t"
-      "mbarrier.arrive.shared::cluster.b64 _, [remote];\n\t}" ::"r"(bar),
-      "r"(rank)
-      : "memory");
 }
 
 }  // namespace

@@ -13,7 +13,7 @@
 // operand of a later kernel.  hook_resid_pre(l) aliases hook_resid_post(l-1) exactly as in the
 // reference cache (the HookPoint is an identity on the same tensor), so it costs no traffic.
 //
-// In fp32 mode with *_lo weight packs present the GEMMs run tcgen05 3xTF32: the A-operand residuals are
+// In fp32 mode with *_lo weight packs present the GEMMs run wgmma 3xTF32: the A-operand residuals are
 // produced by the kernel that produces the operand (LayerNorm out_lo, GEMM out1_lo) or by one
 // pb_split_tf32 pass (patches, z), into f->lo_scratch.
 #include "common.cuh"
@@ -29,7 +29,7 @@ __global__ void __launch_bounds__(256) k_gather_rows(const T* __restrict__ src, 
 
 static int gather_rows(const void* src, int64_t src_ld, void* dst, int rows, int cols, int dtype, cudaStream_t st) {
   int grid = (int)ceil_div64((int64_t)rows * cols, 256);
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > pb_sm_count() * 8) grid = pb_sm_count() * 8;
   if (grid < 1) grid = 1;
   if (dtype == PB_F32) k_gather_rows<float><<<grid, 256, 0, st>>>((const float*)src, src_ld, (float*)dst, rows, cols);
   else k_gather_rows<bf16><<<grid, 256, 0, st>>>((const bf16*)src, src_ld, (bf16*)dst, rows, cols);

@@ -20,14 +20,14 @@ def dtype_code(dtype: torch.dtype) -> int:
     try:
         return _DT[dtype]
     except KeyError:
-        raise L.PrismaB200Error(f"unsupported dtype {dtype}: the B200 path computes in float32 or bfloat16") from None
+        raise L.PrismaB200Error(f"unsupported dtype {dtype}: the H100 path computes in float32 or bfloat16") from None
 
 
 def _need_cuda(*tensors) -> None:
     for t in tensors:
         if t is not None and not t.is_cuda:
             raise L.PrismaB200Error(
-                "prisma_b200 ops need CUDA tensors: the hot path is hand-written sm_100a CUDA and has no CPU fallback "
+                "prisma_b200 ops need CUDA tensors: the hot path is hand-written sm_90a CUDA and has no CPU fallback "
                 f"(got a tensor on {t.device})")
 
 

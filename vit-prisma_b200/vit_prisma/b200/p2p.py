@@ -117,10 +117,9 @@ class P2PGroup:
         import tempfile
         import torch.distributed as dist
         lib = L.get_lib()
-        # Opt-in (PRISMA_P2P_MULTICAST=1).  Measured on 2 and 8 B200s (profiles/r02_dp_notes.md): multimem.ld_reduce makes every GPU
-        # send its WHOLE gradient through its link once (the switch pulls each rank's copy of every slice, the requester's own
-        # included), the peer-load reduce-scatter sends (N-1)/N of it; ingress shrinks to 1/N but the links are full duplex, so the
-        # exchange time is the same at 8 ranks (1.151 vs 1.146 ms/step) and worse at 2 (1.20 vs 1.01).
+        # Opt-in (PRISMA_P2P_MULTICAST=1): multimem.ld_reduce makes every GPU send its WHOLE gradient through its link once (the
+        # switch pulls each rank's copy of every slice, the requester's own included), the peer-load reduce-scatter sends (N-1)/N of
+        # it; ingress shrinks to 1/N but the links are full duplex, so it is not expected to be faster (not measured on H100).
         if os.environ.get("PRISMA_P2P_MULTICAST", "0") != "1" or not (dist.is_available() and dist.is_initialized()):
             self.multicast_note = "NVSwitch multicast available with PRISMA_P2P_MULTICAST=1; not faster than peer loads / stores here"
             return None

@@ -2,7 +2,7 @@
 
 The reference stores attention weights head-major (``W_Q [H, d_model, d_head]``,
 ``W_O [H, d_head, d_model]``; models/layers/attention.py:37-80) and MLP/head weights input-major
-(``W_in [d_model, d_mlp]``; mlp.py:25-36, head.py:19-24).  tcgen05 wants both operands K-major, so
+(``W_in [d_model, d_mlp]``; mlp.py:25-36, head.py:19-24).  wgmma wants both operands K-major, so
 each weight gets a packed ``[N, K]`` shadow copy (plus the tf32 residual ``lo`` in fp32 mode).
 Packs are rebuilt when a parameter's ``_version`` or storage changes (optimizer step,
 ``load_state_dict``, ``.to()``), so the nn.Parameters stay the single source of truth.

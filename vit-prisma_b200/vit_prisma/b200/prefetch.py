@@ -1,6 +1,6 @@
 """Host -> device batch prefetcher: the H2D copy of batch i+1 runs on a copy stream while batch i is in `run_with_cache`.
 
-A 512-image fp32 batch is 308 MB: ~5.6 ms over PCIe gen5, a fifth of a ViT-B/32 all-hooks step on a B200.  The reference
+A 512-image fp32 batch is 308 MB: ~5.6 ms over PCIe gen5 at 55 GB/s, a large share of a ViT-B/32 all-hooks step.  The reference
 feeds its model from a `DataLoader` and `.to(device)` on the compute stream (`activations_store.py:252-270`), i.e. the copy
 sits in front of every forward.  This iterator keeps the same call pattern for the consumer (`for x in prefetcher:
 model.run_with_cache(x)`) and only moves the copy off the critical path: two device buffers, one side stream, event
@@ -17,7 +17,7 @@ class DevicePrefetcher:
     def __init__(self, batches: Optional[Iterable[torch.Tensor]], device: torch.device, depth: int = 2,
                  dtype: Optional[torch.dtype] = None):
         if torch.device(device).type != "cuda":
-            raise RuntimeError("DevicePrefetcher: device must be a CUDA device (the B200 path has no CPU fallback)")
+            raise RuntimeError("DevicePrefetcher: device must be a CUDA device (the H100 path has no CPU fallback)")
         if depth < 2:
             raise ValueError("depth must be >= 2 (one buffer in use, one in flight)")
         self.device = torch.device(device)

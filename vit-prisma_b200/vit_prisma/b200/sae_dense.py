@@ -2,7 +2,7 @@
 
 Stands in for ``StandardSparseAutoencoder.forward`` + ``VisionSAETrainer.train_step`` when ``activation_fn_str == "relu"``
 (the reference's default; sae/sae.py:557-645, 810-839) and for ``_compute_ghost_residual_loss`` (sae/sae.py:151-179) with
-either activation.  The six dense products of the reference graph run on ``pb_gemm`` (tcgen05, 3xTF32, K-major operands:
+either activation.  The six dense products of the reference graph run on ``pb_gemm`` (wgmma, 3xTF32, K-major operands:
 ``pb_transpose`` supplies the transposed views autograd uses); ``csrc/sae_dense.cu`` holds the glue; clip / projection /
 Adam / renorm / dead-feature counters are ``pb_sae_adam``, shared with the TopK pipeline.
 
@@ -158,7 +158,7 @@ class SaeDenseStepEngine(SaeStepEngine):
         WdDT, _ = transpose(WdD, want_lo=False)
         # [rows, d] = exp(h_dead) @ W_dec[dead] (sae.py:165) on the exact-fp32 FFMA kernel: the ghost loss divides by
         # (G - r)^2 / rcn + 1e-6 element-wise, which amplifies round-off in G by ~1e3 (fp32 torch vs fp64: 6e-4 on the
-        # gradients; with the 3xTF32 product here: 4e-2).  Every later ghost product is linear in dL/dG0 and stays on tcgen05.
+        # gradients; with the 3xTF32 product here: 4e-2).  Every later ghost product is linear in dL/dG0 and stays on the tensor cores.
         G0, _ = ops.gemm(E, WdDT, None, impl=L.GEMM_SIMT)
         rsum = colsum(resid)
         L.check(lib.pb_sae_ghost_rows(resid.data_ptr(), rsum.data_ptr(), G0.data_ptr(), self.scalars.data_ptr(), self.aux[1:].data_ptr(),

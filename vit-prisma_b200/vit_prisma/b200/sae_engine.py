@@ -1,6 +1,6 @@
 """TopK-SAE step engine: owns the device buffers of a training step and drives the six C-ABI calls.
 
-    prep -> encoder GEMM (tcgen05 3xTF32 | exact FFMA) -> topk -> decode/loss -> backward -> adam
+    prep -> encoder GEMM (wgmma 3xTF32 | exact FFMA) -> topk -> decode/loss -> backward -> adam
 
 Stands in for ``StandardSparseAutoencoder.forward`` + ``loss.backward()`` + ``clip_grad_norm_`` +
 ``remove_gradient_parallel_to_decoder_directions`` + ``Adam.step`` of the reference
@@ -242,7 +242,7 @@ class SaeStepEngine:
 
     # ------------------------------------------------------------------ pieces
     def _encoder_gemm(self, rows: int) -> None:
-        """hidden_pre = sae_in @ W_enc + b_enc (sae.py:568) on the tcgen05 GEMM (3xTF32) or the exact FFMA kernel."""
+        """hidden_pre = sae_in @ W_enc + b_enc (sae.py:568) on the wgmma GEMM (3xTF32) or the exact FFMA kernel."""
         lib, st = L.get_lib(), _stream()
         use_tc = self.gemm_impl != L.GEMM_SIMT
         g = L.PbGemm()
@@ -306,9 +306,9 @@ class SaeStepEngine:
     # ------------------------------------------------------------------ instrumentation (bench.py / tools)
     def describe_encoder(self) -> str:
         if self.encoder == "fused":
-            return (f"fused: one-pass tf32 tcgen05 GEMM with top-{self.c_keep}-per-128-features epilogue -> exact fp32 re-scoring of "
+            return (f"fused: one-pass tf32 wgmma GEMM with top-{self.c_keep}-per-128-features epilogue -> exact fp32 re-scoring of "
                     f">= {self.m_cand} candidates per token -> exact top-{self.k} with a completeness proof (no dense hidden_pre)")
-        return "tcgen05 3xTF32 GEMM -> dense hidden_pre -> exact k_topk" if self.gemm_impl != L.GEMM_SIMT else "exact FFMA GEMM -> k_topk"
+        return "wgmma 3xTF32 GEMM -> dense hidden_pre -> exact k_topk" if self.gemm_impl != L.GEMM_SIMT else "exact FFMA GEMM -> k_topk"
 
     def fallback_rows(self) -> int:
         """Rows of the last fused encode that took the exact path (host read: synchronises)."""
@@ -329,7 +329,7 @@ class SaeStepEngine:
     def time_stages(self, x: torch.Tensor, lr: float, since_fired=None, act_freq=None, reps: int = 5) -> dict:
         """CUDA-event time of every stage of one training step, each replayed ``reps`` times back to back on the current stream
         (warm caches: shares of the step, not cold-start figures).  Mutates parameters / optimizer state like ``reps`` extra steps.
-        Returns ``{stage: {"ms", "bytes" | "flops" (algorithmic, per launch), "ncu" (kernel-name regex for profiles/)}}``."""
+        Returns ``{stage: {"ms", "bytes" | "flops" (algorithmic, per launch), "ncu" (kernel-name regex for a stored ncu summary)}}``."""
         lib, st = L.get_lib(), _stream()
         x = ops_cast_f32(x)
         rows = x.shape[0]
@@ -378,7 +378,7 @@ class SaeStepEngine:
                     ("select + exact re-score alone", lambda: L.check(lib.pb_sae_encode_topk_fused(C.byref(self._enc_desc(rows, 2)), st)),
                      dict(bytes=4 * rows * nkeys + 4 * rows * self.d + 8 * rows * self.k, ncu=r"k_cand_select"))]
         return [("encode + topk (prep + encoder GEMM 3xTF32 + exact topk)", lambda: self.encode_topk(x),
-                 dict(flops=2.0 * rows * self.d * self.F, passes=3, ncu=r"k_gemm_tc2<float")),
+                 dict(flops=2.0 * rows * self.d * self.F, passes=3, ncu=r"k_gemm_tc<float")),
                 ("encoder GEMM alone (hidden_pre = sae_in @ W_enc + b_enc)", lambda: self._encoder_gemm(rows),
                  dict(flops=2.0 * rows * self.d * self.F, passes=3, bytes=8 * self.d * self.F + 8 * rows * self.d + 4 * rows * self.F))]
 

@@ -7,7 +7,7 @@ with ``layer_acts[:, 0]`` as the input activation and ``layer_acts[:, 1]`` as th
     sae_out     = norm_out(out_n)   with the INPUT's row statistics           (:81)
     loss        = mean((sae_out - y)^2 / ||y - mean_batch(y)||) + l1           (:83, 93-103; l1 only for dense activations)
 
-The dense products run on ``pb_gemm`` (3xTF32 tcgen05) exactly as in ``SaeDenseStepEngine``; this module adds the target-vs-input
+The dense products run on ``pb_gemm`` (3xTF32 wgmma) exactly as in ``SaeDenseStepEngine``; this module adds the target-vs-input
 split of the loss, the skip matrix (one more forward product through the residual epilogue, one more gradient product) and the
 second decoder bias.  ``pb_sae_adam`` updates W_dec (clip, decoder-parallel-gradient removal, Adam, row renorm), W_enc, b_enc and
 b_dec; ``pb_adam_vec`` updates W_skip and b_dec_out with the same clip coefficient.  Requires d_out == d_in (the reference default).
@@ -40,9 +40,9 @@ class SaeTranscoderStepEngine(SaeDenseStepEngine):
                  l1_coefficient: float = 0.0, **kw):
         super().__init__(W_encT, W_dec, b_enc, b_dec, k=max(int(k), 1), l1_coefficient=l1_coefficient, **kw)
         if W_dec.shape[1] != self.d:
-            raise L.PrismaB200Error("B200 transcoder step: d_out must equal d_in")
+            raise L.PrismaB200Error("H100 transcoder step: d_out must equal d_in")
         if activation not in ("relu", "topk"):
-            raise NotImplementedError(f"B200 transcoder step: activation {activation!r} is not built (relu and topk are)")
+            raise NotImplementedError(f"H100 transcoder step: activation {activation!r} is not built (relu and topk are)")
         _need_cuda(b_dec_out, W_skip)
         self.activation, self.b_dec_out, self.W_skip = activation, b_dec_out, W_skip
         dev, d = W_dec.device, self.d

@@ -1,6 +1,6 @@
 """Host-resident modules on a GPU-only compute path.
 
-Device policy of this package: every arithmetic operation runs in the sm_100a kernels; there is no CPU compute path.  The reference's
+Device policy of this package: every arithmetic operation runs in the sm_90a kernels; there is no CPU compute path.  The reference's
 default ``HookedViTConfig.device`` is ``"cpu"`` and its own offline tests build host-resident models / layers and feed host tensors.
 Such a module is *staged*: for the duration of one call its parameters and buffers point at cached device copies (refreshed when a
 parameter's version counter or storage changes), tensor arguments are copied host -> device, the same CUDA kernels run, and tensor
@@ -34,7 +34,7 @@ def staged_on_gpu(module: torch.nn.Module):
     """Point every host parameter / buffer of ``module`` at a cached device copy for the duration of the block."""
     if not torch.cuda.is_available():
         raise PrismaB200Error("prisma_b200: this module lives in host memory and no CUDA device is visible -- the hot path is "
-                              "hand-written sm_100a CUDA and has no CPU fallback")
+                              "hand-written sm_90a CUDA and has no CPU fallback")
     cache = module.__dict__.setdefault("_stage_cache", {})
     swapped = []
     for name, t in list(module.named_parameters()) + list(module.named_buffers()):

@@ -3,7 +3,7 @@
 The constructor signature is API: the reference's callers (and its tests) build the config positionally,
 ``HookedViTConfig(n_layers, d_model, d_head, d_mlp, ...)``, and by keyword with every name below
 (reference: src/vit_prisma/configs/HookedViTConfig.py:8-123).  The record is generated from one table so that the order,
-the names and the defaults live in a single place; what the B200 engine does with each group:
+the names and the defaults live in a single place; what the H100 engine does with each group:
 
   geometry      -> sizes baked into kernel launch descriptors (PbVitForward)
   graph toggles -> select the fused chain vs. the module-by-module hooked route
@@ -115,7 +115,7 @@ _FIELDS = [
     ("save_dir", str, "Checkpoints"),
     ("save_checkpoints", bool, True),
     ("save_cp_frequency", int, 5),
-    # video (tubelet) towers: accepted, not on the B200 hot path
+    # video (tubelet) towers: accepted, not on the H100 hot path
     ("is_video_transformer", bool, False),
     ("video_tubelet_depth", Optional[int], None),
     ("video_num_frames", Optional[int], None),

@@ -1,4 +1,4 @@
-"""Activation names understood by the B200 ops (reference models/activation_fns.py:19-57, mlp.py:41-62).
+"""Activation names understood by the H100 ops (reference models/activation_fns.py:19-57, mlp.py:41-62).
 
 The closed forms are evaluated inside the CUDA kernels (csrc/common.cuh ``apply_act``); this module
 only maps ``HookedViTConfig.activation_name`` to the kernel's activation code and implements

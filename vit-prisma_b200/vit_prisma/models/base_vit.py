@@ -1,4 +1,4 @@
-"""HookedViT -- the hooked vision transformer, B200-native (reference models/base_vit.py:60-824).
+"""HookedViT -- the hooked vision transformer, H100-native (reference models/base_vit.py:60-824).
 
 Two execution routes produce the same numbers from the same kernels:
 

@@ -42,7 +42,7 @@ class PatchEmbedding(nn.Module):
 
 
 class TubeletEmbedding(nn.Module):
-    """Video tubelet embedding (reference :36-62).  Parameter container only: the B200 hot path covers
+    """Video tubelet embedding (reference :36-62).  Parameter container only: the H100 hot path covers
     image towers; calling it raises instead of silently running somewhere else."""
 
     def __init__(self, cfg):
@@ -53,4 +53,4 @@ class TubeletEmbedding(nn.Module):
 
     @host_staged
     def forward(self, x):
-        raise NotImplementedError("TubeletEmbedding (video) is outside the B200 hot-path scope (SURVEY #6)")
+        raise NotImplementedError("TubeletEmbedding (video) is outside the H100 hot-path scope (SURVEY #6)")

@@ -8,7 +8,7 @@ residual-stream analysis helpers (``accumulated_resid``, ``decompose_resid``,
 PyTorch post-processing -- they run on whatever device the cached tensors live on and are
 not kernel targets.
 
-On the fused B200 path the values are *views into one cache arena* written by the CUDA
+On the fused H100 path the values are *views into one cache arena* written by the CUDA
 chain (see vit_prisma/b200/vit_engine.py); the views own the arena, so it lives exactly
 as long as any cached tensor does.
 """

@@ -1,7 +1,7 @@
 """FactoredMatrix -- low-rank product ``A @ B`` kept in factored form.
 
 Analysis-side utility (reference src/vit_prisma/prisma_tools/factored_matrix.py:22-245,
-out of the B200 hot-path scope, SURVEY #22); provided so ``Attention.OV`` /
+out of the H100 hot-path scope, SURVEY #22); provided so ``Attention.OV`` /
 ``Attention.QK`` and ``HookedViT.fold_value_biases``-style post-processing keep
 working.  Plain PyTorch -- it never touches the activation path.
 """

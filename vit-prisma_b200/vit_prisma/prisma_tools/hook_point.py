@@ -8,7 +8,7 @@ Behavioural contract taken from reference src/vit_prisma/prisma_tools/hook_point
 * ``add_hook(hook, dir, is_permanent, level, prepend)``, ``add_perma_hook``,
   ``remove_hooks(dir, including_permanent, level)``, ``clear_context``, ``layer()``.
 
-B200 notes.  On the fused fast path (``HookedViT.run_with_cache`` with nothing
+H100 notes.  On the fused fast path (``HookedViT.run_with_cache`` with nothing
 but the internal save-hook attached) HookPoints are never *called*: the CUDA
 chain writes every requested activation straight into the cache arena and the
 Python side only builds the key -> view dictionary.  On the per-op hooked path

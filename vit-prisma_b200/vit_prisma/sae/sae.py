@@ -1,4 +1,4 @@
-"""Sparse autoencoders on the B200 path (reference sae/sae.py:29-839).
+"""Sparse autoencoders on the H100 path (reference sae/sae.py:29-839).
 
 ``StandardSparseAutoencoder`` keeps the reference surface -- ``encode`` / ``decode`` / ``forward`` (7-tuple),
 ``set_decoder_norm_to_unit_norm``, ``initialize_b_dec*``, ``save_model`` / ``load_from_pretrained``, the four
@@ -49,7 +49,7 @@ class TopK(nn.Module):
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         from vit_prisma.b200.sae_engine import topk_dense
         if not isinstance(self.postact_fn, nn.ReLU):
-            raise NotImplementedError("TopK on the B200 path supports the default ReLU post-activation")
+            raise NotImplementedError("TopK on the H100 path supports the default ReLU post-activation")
         return topk_dense(x, self.k)
 
 
@@ -305,9 +305,9 @@ class StandardSparseAutoencoder(SparseAutoencoder):
         from vit_prisma.b200.sae_engine import SaeStepEngine
         act = self.cfg.activation_fn_str
         if act not in ("topk", "relu"):
-            raise NotImplementedError(f"B200 training step: activation_fn_str {act!r} is not built (topk and relu are)")
+            raise NotImplementedError(f"H100 training step: activation_fn_str {act!r} is not built (topk and relu are)")
         if act == "relu" and getattr(self.cfg, "lp_norm", 1) != 1:
-            raise NotImplementedError("B200 dense training step: only lp_norm == 1 (the reference default) is built")
+            raise NotImplementedError("H100 dense training step: only lp_norm == 1 (the reference default) is built")
         dense = act == "relu" or bool(self.cfg.use_ghost_grads)
         wt, wd, be, bd = self._engine_params()
         eng = self._engine
@@ -465,9 +465,9 @@ class GatedSparseAutoencoder(SparseAutoencoder):
         super().__init__(cfg)
         assert self.cfg.use_ghost_grads == False, "Gated SAE does not support ghost grads"   # noqa: E712  (reference :655-657)
         if cfg.activation_fn_str != "relu":
-            raise NotImplementedError("B200 Gated SAE: activation_fn_str must be 'relu' (the reference default)")
+            raise NotImplementedError("H100 Gated SAE: activation_fn_str must be 'relu' (the reference default)")
         if self.dtype != torch.float32:
-            raise NotImplementedError("B200 Gated SAE runs in float32")
+            raise NotImplementedError("H100 Gated SAE runs in float32")
 
     def initialize_sae_weights(self):                                     # reference :659-693 (plain kaiming_uniform_, no row norm)
         enc = torch.nn.init.kaiming_uniform_(torch.empty(self.cfg.d_in, self.cfg.d_sae, dtype=self.dtype, device=self.device))
@@ -502,7 +502,7 @@ class GatedSparseAutoencoder(SparseAutoencoder):
     def _fire(self, hook: HookPoint, t: torch.Tensor) -> torch.Tensor:
         out = hook(t)
         if out is not t and out.data_ptr() != t.data_ptr():
-            raise NotImplementedError("B200 Gated SAE: hooks may observe activations but not replace them")
+            raise NotImplementedError("H100 Gated SAE: hooks may observe activations but not replace them")
         return t
 
     def _run(self, x: torch.Tensor):

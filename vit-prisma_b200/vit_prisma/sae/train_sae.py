@@ -1,4 +1,4 @@
-"""VisionSAETrainer -- SAE training entry point on the B200 path (reference sae/train_sae.py:61-861).
+"""VisionSAETrainer -- SAE training entry point on the H100 path (reference sae/train_sae.py:61-861).
 
 Same constructor, ``run()`` / ``train_step(...)`` / ``checkpoint(...)`` surface and the same order of operations per
 step (train_sae.py:278-411):

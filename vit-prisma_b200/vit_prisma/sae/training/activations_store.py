@@ -2,7 +2,7 @@
 
 ``VisionActivationsStore`` keeps the reference's interface and mixing semantics -- a storage half-buffer, refills of
 ``n_batches_in_buffer // 2`` image batches through ``model.run_with_cache(names_filter=[hook], stop_at_layer=layer+1)``,
-concatenate + ``randperm`` shuffle, keep half, serve half -- with two B200-minded changes:
+concatenate + ``randperm`` shuffle, keep half, serve half -- with two H100-minded changes:
 
 * refills hit the fused ViT chain with a one-key ``names_filter`` (nothing but the requested hook point is spilled,
   blocks after the hook layer are never launched);

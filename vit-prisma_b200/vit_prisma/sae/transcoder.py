@@ -1,9 +1,9 @@
-"""Transcoder on the B200 path (reference sae/transcoder.py:6-116): a sparse coder whose decoder reconstructs a DIFFERENT
+"""Transcoder on the H100 path (reference sae/transcoder.py:6-116): a sparse coder whose decoder reconstructs a DIFFERENT
 activation (``cfg.out_hook_point``, e.g. the MLP output) from the one it encodes, optionally with a linear skip connection.
 
 Same surface as the reference class -- parameters ``W_skip [d_in, d_in] | None``, ``W_dec [d_sae, d_out]``, ``W_enc [d_in, d_sae]``,
 ``b_enc``, ``b_dec``, ``b_dec_out``; ``encode`` / ``decode`` / ``forward(x, y, dead_neuron_mask)`` -> 7-tuple -- on top of
-``vit_prisma/b200/sae_transcoder.py`` (dense 3xTF32 tcgen05 products + the shared Adam kernels).  ``forward`` builds no autograd graph;
+``vit_prisma/b200/sae_transcoder.py`` (dense 3xTF32 wgmma products + the shared Adam kernels).  ``forward`` builds no autograd graph;
 ``VisionSAETrainer`` trains through the engine's hand-written backward.  Ghost grads are not built for this class."""
 from __future__ import annotations
 
@@ -19,7 +19,7 @@ class Transcoder(SparseAutoencoder):
     def initialize_sae_weights(self):                                     # reference :8-29, same order of random draws
         cfg = self.cfg
         if getattr(cfg, "d_out", self.d_in) != self.d_in:
-            raise NotImplementedError("B200 Transcoder: d_out must equal d_in (the reference default)")
+            raise NotImplementedError("H100 Transcoder: d_out must equal d_in (the reference default)")
         self.W_skip = nn.Parameter(self.initialize_weights(self.d_in, self.d_in)) if cfg.transcoder_with_skip_connection else None
         self.W_dec = nn.Parameter(self.initialize_weights(self.d_sae, cfg.d_out))
         enc = self.initialize_weights(self.d_in, self.d_sae)                # [d_in, d_sae], rows unit-norm
@@ -40,9 +40,9 @@ class Transcoder(SparseAutoencoder):
     def step_engine(self, gemm_impl: int = L.GEMM_AUTO):
         from vit_prisma.b200.sae_transcoder import SaeTranscoderStepEngine
         if self.cfg.use_ghost_grads:
-            raise NotImplementedError("B200 Transcoder: ghost grads are not built")
+            raise NotImplementedError("H100 Transcoder: ghost grads are not built")
         if self.dtype != torch.float32:
-            raise NotImplementedError("B200 Transcoder runs in float32")
+            raise NotImplementedError("H100 Transcoder runs in float32")
         params = self._canonical_params()
         key = tuple(0 if t is None else t.data_ptr() for t in params) + (gemm_impl,)
         eng = self._engine
