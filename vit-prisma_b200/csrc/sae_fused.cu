@@ -3,12 +3,12 @@
 //
 // Approximate-then-rescore, exact by construction:
 //   1. k_enc_cand     persistent wgmma GEMM, ONE tf32 pass (the fp32 operands are read by the tensor core with their 13 low
-//                     mantissa bits ignored), 128 x 128 tiles: a tile's columns are one 128-feature segment.  The epilogue never
-//                     stores the tile: every thread keeps the C_KEEP largest of the 32 values it holds of each of its two token
-//                     rows as packed keys (order-preserving int of the value, the low 7 bits replaced by the column inside the
-//                     segment) with a branch-free insertion network, the four threads sharing a row merge their lists by
-//                     shuffles, and one of them writes C_KEEP x 4 bytes.  Per token: d_sae / 128 segments x C_KEEP keys (6 KB at
-//                     d_sae = 24576) instead of a 98 KB dense row.
+//                     mantissa bits ignored), 128 x 256 tiles: a tile's columns are two 128-feature segments.  The epilogue never
+//                     stores the tile: per segment, every thread turns the 32 values it holds of each of its two token rows into
+//                     packed keys (order-preserving int of the value, the low 7 bits replaced by the column inside the segment)
+//                     and keeps the 8 largest with sorting networks, the four threads sharing a row merge their lists by
+//                     shuffles, and one of them writes the first C_KEEP x 4 bytes.  Per token: d_sae / 128 segments x C_KEEP keys
+//                     (6 KB at d_sae = 24576) instead of a 98 KB dense row.
 //   2. k_cand_select  one CTA per token: the m_cand best keys of the row (threshold from per-thread bests, rank by counting),
 //                     EXACT fp32 re-evaluation of those m_cand pre-activations (FFMA dot products against W_encT rows),
 //                     exact top-k of the re-scored values (ties -> lower index, sorted descending), and a proof that no
@@ -32,42 +32,66 @@ __device__ __forceinline__ int f2ord(float v) {           // monotone float -> s
 __device__ __forceinline__ float ord2f(int k) { return __int_as_float(k ^ ((k >> 31) & 0x7fffffff)); }
 __device__ __forceinline__ bool key_gt_f(float va, int ia, float vb, int ib) { return va > vb || (va == vb && ia < ib); }
 
-constexpr int FZ_SEG = 128;      // columns per segment = tile columns (TC_BN)
-constexpr int FZ_STAGES = 6;     // 6 x (16 KB A + 16 KB B) = 192 KB operand ring
-using FzCfg = TcCfg<float, 1, FZ_STAGES>;
-constexpr int FZ_SMEM = FzCfg::RING_BYTES + 1024 + 256;
-static_assert(FZ_SEG == TC_BN, "a tile is one segment");
+constexpr int FZ_SEG = 128;                       // features per segment: the keys of a segment carry the column in 7 bits
+constexpr int FZ_BM = 128;                        // tile rows: two consumer warpgroups of 64 tokens
+constexpr int FZ_BN = 2 * FZ_SEG;                 // tile columns: two segments, one m64n256 accumulator (128 registers) per thread
+constexpr int FZ_BK = 32;                         // fp32 elements per 128-byte k-slab
+constexpr int FZ_KSTEPS = 4;                      // one wgmma consumes 8 fp32 (32 bytes) of K per row
+constexpr int FZ_A_BYTES = FZ_BM * 128;           // 16 KB
+constexpr int FZ_STAGE_BYTES = FZ_A_BYTES + FZ_BN * 128;   // + 32 KB of W_encT
+constexpr int FZ_STAGES = 4;                      // 4 x 48 KB = 192 KB operand ring
+constexpr int FZ_SMEM = FZ_STAGES * FZ_STAGE_BYTES + 1024 + 256;
 
-__device__ __forceinline__ void key_insert(int (&s)[8], int x, int n) {   // s[0, n) stays sorted descending
+// ---- top-8 of a thread's keys by sorting networks (keys are distinct: the column sits in the low 7 bits)
+__device__ __forceinline__ void key_cas(int& a, int& b) {   // a >= b afterwards
+  const int hi = max(a, b);
+  b = min(a, b);
+  a = hi;
+}
+// v[0, 8) sorted descending: the optimal 19-comparator network for 8 inputs
+__device__ __forceinline__ void key_sort8(int* v) {
+  key_cas(v[0], v[2]); key_cas(v[1], v[3]); key_cas(v[4], v[6]); key_cas(v[5], v[7]);
+  key_cas(v[0], v[4]); key_cas(v[1], v[5]); key_cas(v[2], v[6]); key_cas(v[3], v[7]);
+  key_cas(v[0], v[1]); key_cas(v[2], v[3]); key_cas(v[4], v[5]); key_cas(v[6], v[7]);
+  key_cas(v[2], v[4]); key_cas(v[3], v[5]);
+  key_cas(v[1], v[4]); key_cas(v[3], v[6]);
+  key_cas(v[1], v[2]); key_cas(v[3], v[4]); key_cas(v[5], v[6]);
+}
+// a, b sorted descending -> a = the 8 largest of both, sorted descending: a half-cleaner against reversed b leaves the top 8 as a
+// bitonic sequence, which 12 comparators sort
+__device__ __forceinline__ void key_merge8(int* a, const int* b) {
 #pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    if (i < n) {
-      const int hi = max(s[i], x);
-      x = min(s[i], x);
-      s[i] = hi;
-    }
-  }
+  for (int i = 0; i < 8; ++i) a[i] = max(a[i], b[7 - i]);
+  key_cas(a[0], a[4]); key_cas(a[1], a[5]); key_cas(a[2], a[6]); key_cas(a[3], a[7]);
+  key_cas(a[0], a[2]); key_cas(a[1], a[3]); key_cas(a[4], a[6]); key_cas(a[5], a[7]);
+  key_cas(a[0], a[1]); key_cas(a[2], a[3]); key_cas(a[4], a[5]); key_cas(a[6], a[7]);
+}
+// v[0, 32) -> v[0, 8) = the 8 largest, sorted descending
+__device__ __forceinline__ void key_top8_of32(int (&v)[32]) {
+  key_sort8(v); key_sort8(v + 8); key_sort8(v + 16); key_sort8(v + 24);
+  key_merge8(v, v + 8);
+  key_merge8(v + 16, v + 24);
+  key_merge8(v, v + 16);
 }
 
 template <int C_KEEP>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 k_enc_cand(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, int K, int M, int N,
            const float* __restrict__ bias, int* __restrict__ cand, int num_m_tiles, int num_n_tiles) {
-  using C = FzCfg;
   pb_pdl_trigger();
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem0 = smem_u32(smem_raw);
   const uint32_t ring = (smem0 + 1023u) & ~1023u;
-  const uint32_t bar_base = ring + C::RING_BYTES;
+  const uint32_t bar_base = ring + FZ_STAGES * FZ_STAGE_BYTES;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (FZ_STAGES + s); };
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int wg = warp >> 2;
-  const int num_kb = (K + C::BK - 1) / C::BK;
+  const int num_kb = (K + FZ_BK - 1) / FZ_BK;
   const int num_tiles = num_m_tiles * num_n_tiles;
   const int nseg = N / FZ_SEG;
-  // m-fastest raster: the CTAs in flight share one 128-feature slab of the dictionary and walk the token tiles, so W_encT
+  // m-fastest raster: the CTAs in flight share one 256-feature slab of the dictionary and walk the token tiles, so W_encT
   // (75 MB at d_sae = 24576) streams from HBM once while sae_in (12.6 MB) stays L2-resident.
   auto tile_m = [&](int tile) { return tile % num_m_tiles; };
   auto tile_n = [&](int tile) { return tile / num_m_tiles; };
@@ -87,37 +111,37 @@ k_enc_cand(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
     if (threadIdx.x == 0) {
       uint32_t it = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int m0 = tile_m(tile) * TC_BM, n0 = tile_n(tile) * TC_BN;
+        const int m0 = tile_m(tile) * FZ_BM, n0 = tile_n(tile) * FZ_BN;
         for (int kb = 0; kb < num_kb; ++kb, ++it) {
           const int s = it % FZ_STAGES;
           const uint32_t ph = (it / FZ_STAGES) & 1;
           mbar_wait<false>(empty_bar(s), ph ^ 1);
-          mbar_expect_tx(full_bar(s), C::STAGE_BYTES);
-          const uint32_t sa = ring + s * C::STAGE_BYTES;
-          tma_load_2d(sa, &tmA, full_bar(s), kb * C::BK, m0);
-          tma_load_2d(sa + C::A_BYTES, &tmB, full_bar(s), kb * C::BK, n0);
+          mbar_expect_tx(full_bar(s), FZ_STAGE_BYTES);       // a box reaching past M or F still delivers (zero-filled) full bytes
+          const uint32_t sa = ring + s * FZ_STAGE_BYTES;
+          tma_load_2d(sa, &tmA, full_bar(s), kb * FZ_BK, m0);
+          tma_load_2d(sa + FZ_A_BYTES, &tmB, full_bar(s), kb * FZ_BK, n0);
         }
       }
     }
     return;
   }
-  // ===================== consumers: one tf32 pass, then per-row top-C_KEEP of the segment as packed keys =====================
+  // ===================== consumers: one tf32 pass, then per-row top-C_KEEP of each segment as packed keys =====================
   reg_alloc<232>();
   const int c = wg - 1, wq = warp & 3, tid = threadIdx.x & 127;
-  float acc[64];
+  float acc[128];
   uint32_t it = 0;
   for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-    const int m0 = tile_m(tile) * TC_BM, n0 = tile_n(tile) * TC_BN;
+    const int m0 = tile_m(tile) * FZ_BM, n0 = tile_n(tile) * FZ_BN;
     int prev_s = -1;
     for (int kb = 0; kb < num_kb; ++kb, ++it) {
       const int s = it % FZ_STAGES;
       const uint32_t ph = (it / FZ_STAGES) & 1;
       mbar_wait<false>(full_bar(s), ph);
-      const uint32_t sa = ring + s * C::STAGE_BYTES + c * 64 * 128;
-      const uint32_t sb = ring + s * C::STAGE_BYTES + C::A_BYTES;
+      const uint32_t sa = ring + s * FZ_STAGE_BYTES + c * 64 * 128;
+      const uint32_t sb = ring + s * FZ_STAGE_BYTES + FZ_A_BYTES;
       wgmma_fence();
 #pragma unroll
-      for (int k = 0; k < C::KSTEPS; ++k) wgmma_tf32_n128(acc, make_smem_desc(sa + 32 * k), make_smem_desc(sb + 32 * k), (kb | k) != 0 ? 1u : 0u);
+      for (int k = 0; k < FZ_KSTEPS; ++k) wgmma_tf32_n256(acc, make_smem_desc(sa + 32 * k), make_smem_desc(sb + 32 * k), (kb | k) != 0 ? 1u : 0u);
       wgmma_commit();
       wgmma_wait<1>();
       if (prev_s >= 0 && tid == 0) mbar_arrive(empty_bar(prev_s));
@@ -127,41 +151,48 @@ k_enc_cand(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
     wgmma_fence_acc(acc);
     if (tid == 0) mbar_arrive(empty_bar(prev_s));
 
-    // accumulator element i of this thread: row 16 wq + lane / 4 + 8 ((i >> 1) & 1), column 8 (i >> 2) + 2 (lane % 4) + (i & 1)
-    int s0[8], s1[8];
+    // accumulator element i of this thread: row 16 wq + lane / 4 + 8 ((i >> 1) & 1), column 8 (i >> 2) + 2 (lane % 4) + (i & 1);
+    // segment g of the tile is elements [64 g, 64 g + 64).  Only one segment's key lists are live at a time.
+    const int row = m0 + 64 * c + 16 * wq + (lane >> 2);
 #pragma unroll
-    for (int i = 0; i < 8; ++i) { s0[i] = INT_MIN; s1[i] = INT_MIN; }
+    for (int g = 0; g < 2; ++g) {
+      const int f0 = n0 + g * FZ_SEG;
+      if (f0 >= N) break;                            // F is a multiple of 128, not of 256: the last tile's second half is empty
+      int s0[32], s1[32];
 #pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      const int col = 8 * j + 2 * (lane & 3);
-      const float2 bb = *reinterpret_cast<const float2*>(bias + n0 + col);
-      key_insert(s0, (f2ord(acc[4 * j] + bb.x) & ~127) | col, C_KEEP);
-      key_insert(s0, (f2ord(acc[4 * j + 1] + bb.y) & ~127) | (col + 1), C_KEEP);
-      key_insert(s1, (f2ord(acc[4 * j + 2] + bb.x) & ~127) | col, C_KEEP);
-      key_insert(s1, (f2ord(acc[4 * j + 3] + bb.y) & ~127) | (col + 1), C_KEEP);
-    }
-    // the four lanes of a quad hold disjoint columns of the same two rows: merge their lists (keys are distinct)
+      for (int j = 0; j < 16; ++j) {
+        const int col = 8 * j + 2 * (lane & 3);
+        const float2 bb = *reinterpret_cast<const float2*>(bias + f0 + col);
+        const float* a = acc + 64 * g + 4 * j;
+        s0[2 * j] = (f2ord(a[0] + bb.x) & ~127) | col;
+        s0[2 * j + 1] = (f2ord(a[1] + bb.y) & ~127) | (col + 1);
+        s1[2 * j] = (f2ord(a[2] + bb.x) & ~127) | col;
+        s1[2 * j + 1] = (f2ord(a[3] + bb.y) & ~127) | (col + 1);
+      }
+      key_top8_of32(s0);
+      key_top8_of32(s1);
+      // the four lanes of a quad hold disjoint columns of the same two rows: merge their lists (keys are distinct)
 #pragma unroll
-    for (int off = 1; off <= 2; off <<= 1) {
-      int t0[8], t1[8];
+      for (int off = 1; off <= 2; off <<= 1) {
+        int t0[8], t1[8];
 #pragma unroll
-      for (int i = 0; i < C_KEEP; ++i) { t0[i] = __shfl_xor_sync(0xffffffffu, s0[i], off); t1[i] = __shfl_xor_sync(0xffffffffu, s1[i], off); }
+        for (int i = 0; i < 8; ++i) { t0[i] = __shfl_xor_sync(0xffffffffu, s0[i], off); t1[i] = __shfl_xor_sync(0xffffffffu, s1[i], off); }
+        key_merge8(s0, t0);
+        key_merge8(s1, t1);
+      }
+      if ((lane & 3) == 0) {
 #pragma unroll
-      for (int i = 0; i < C_KEEP; ++i) { key_insert(s0, t0[i], C_KEEP); key_insert(s1, t1[i], C_KEEP); }
-    }
-    if ((lane & 3) == 0) {
-      const int row = m0 + 64 * c + 16 * wq + (lane >> 2);
+        for (int h = 0; h < 2; ++h) {
+          const int* sv = h == 0 ? s0 : s1;
+          if (row + 8 * h < M) {
+            int* dst = cand + ((int64_t)(row + 8 * h) * nseg + f0 / FZ_SEG) * C_KEEP;
+            if (C_KEEP % 4 == 0) {
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int* sv = h == 0 ? s0 : s1;
-        if (row + 8 * h < M) {
-          int* dst = cand + ((int64_t)(row + 8 * h) * nseg + n0 / FZ_SEG) * C_KEEP;
-          if (C_KEEP % 4 == 0) {
+              for (int i = 0; i < C_KEEP / 4; ++i) reinterpret_cast<int4*>(dst)[i] = make_int4(sv[4 * i], sv[4 * i + 1], sv[4 * i + 2], sv[4 * i + 3]);
+            } else {
 #pragma unroll
-            for (int i = 0; i < C_KEEP / 4; ++i) reinterpret_cast<int4*>(dst)[i] = make_int4(sv[4 * i], sv[4 * i + 1], sv[4 * i + 2], sv[4 * i + 3]);
-          } else {
-#pragma unroll
-            for (int i = 0; i < C_KEEP / 2; ++i) reinterpret_cast<int2*>(dst)[i] = make_int2(sv[2 * i], sv[2 * i + 1]);
+              for (int i = 0; i < C_KEEP / 2; ++i) reinterpret_cast<int2*>(dst)[i] = make_int2(sv[2 * i], sv[2 * i + 1]);
+            }
           }
         }
       }
@@ -512,15 +543,15 @@ __global__ void __launch_bounds__(256) k_rownorm_max(const float* __restrict__ W
 template <int C_KEEP>
 int launch_enc_cand(const PbSaeEncode* e, cudaStream_t st) {
   CUtensorMap tmA, tmB;
-  PB_TRY(make_map(&tmA, e->sae_in, PB_F32, e->rows, e->d, e->d, TC_BM));
-  PB_TRY(make_map(&tmB, e->W_encT, PB_F32, e->F, e->d, e->d, TC_BN));
+  PB_TRY(make_map(&tmA, e->sae_in, PB_F32, e->rows, e->d, e->d, FZ_BM));
+  PB_TRY(make_map(&tmB, e->W_encT, PB_F32, e->F, e->d, e->d, FZ_BN));
   auto kern = k_enc_cand<C_KEEP>;
   static bool attr_done = false;
   if (!attr_done) {
     PB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, FZ_SMEM));
     attr_done = true;
   }
-  const int num_m = (e->rows + TC_BM - 1) / TC_BM, num_n = (e->F + TC_BN - 1) / TC_BN;
+  const int num_m = (e->rows + FZ_BM - 1) / FZ_BM, num_n = (e->F + FZ_BN - 1) / FZ_BN;
   int grid = pb_sm_count();
   if (grid > num_m * num_n) grid = num_m * num_n;
   PB_LAUNCH_PDL(kern, grid, TC_THREADS, FZ_SMEM, st, tmA, tmB, e->d, e->rows, e->F, e->b_enc, e->cand, num_m, num_n);
