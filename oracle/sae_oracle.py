@@ -44,19 +44,26 @@ def normalise_in(x: torch.Tensor, mode: str, eps: float = 1e-5):
 
 def sae_forward(p: Dict[str, torch.Tensor], x: torch.Tensor, k: int, mode: str = "layer_norm", xbar: Optional[torch.Tensor] = None,
                 global_rows: Optional[int] = None, act: str = "topk", l1_coefficient: float = 0.0,
-                dead_mask: Optional[torch.Tensor] = None) -> Dict[str, torch.Tensor]:
+                dead_mask: Optional[torch.Tensor] = None, topk_idx: Optional[torch.Tensor] = None,
+                topk_val: Optional[torch.Tensor] = None) -> Dict[str, torch.Tensor]:
     """p: W_enc [d,F], W_dec [F,d], b_enc [F], b_dec [d].
     ``xbar`` / ``global_rows``: data-parallel shard view -- batch mean and token count of the GLOBAL batch, so that the
     shard's loss share and gradients sum over shards to the single-process values.
-    ``act``: "topk" | "relu".  ``dead_mask`` [F] bool (not None <=> cfg.use_ghost_grads in training mode): ghost term."""
+    ``act``: "topk" | "relu".  ``dead_mask`` [F] bool (not None <=> cfg.use_ghost_grads in training mode): ghost term.
+    ``topk_idx`` [rows, k] (and ``topk_val``): take this TopK selection (and these pre-activation values) instead of
+    torch.topk's, so that the rest of the step can be checked on the same support as an implementation whose fp32
+    selection legitimately differs in a near-tie row."""
     xn, mu, std = normalise_in(x, mode)
     sae_in = xn - p["b_dec"]                            # sae.py:564-566
     hidden_pre = sae_in @ p["W_enc"] + p["b_enc"]      # :568-574
     if act == "topk":
-        top = torch.topk(hidden_pre, k=k, dim=-1)       # :803-805
-        vals = torch.relu(top.values)
-        feature_acts = torch.zeros_like(hidden_pre).scatter_(-1, top.indices, vals)   # :806-808
-        idx, raw_val = top.indices, top.values
+        if topk_idx is None:
+            top = torch.topk(hidden_pre, k=k, dim=-1)   # :803-805
+            idx, raw_val = top.indices, top.values
+        else:
+            idx = topk_idx.to(hidden_pre.device).long()
+            raw_val = hidden_pre.gather(-1, idx) if topk_val is None else topk_val.to(hidden_pre)
+        feature_acts = torch.zeros_like(hidden_pre).scatter_(-1, idx, torch.relu(raw_val))   # :806-808
     elif act == "relu":
         feature_acts = torch.relu(hidden_pre)           # :810-839 get_activation_fn("relu")
         idx = raw_val = None
@@ -128,11 +135,13 @@ def new_adam_state(p: Dict[str, torch.Tensor]) -> Dict[str, Dict[str, torch.Tens
 def sae_train_step(p: Dict[str, torch.Tensor], state, x: torch.Tensor, k: int, lr: float, t: int, mode: str = "layer_norm",
                    max_grad_norm: Optional[float] = 1.0, betas=(0.9, 0.999), eps: float = 1e-8,
                    since_fired: Optional[torch.Tensor] = None, act_freq: Optional[torch.Tensor] = None, act: str = "topk",
-                   l1_coefficient: float = 0.0, use_ghost_grads: bool = False, dead_feature_window: int = 5000):
-    """One reference train_step (train_sae.py:278-411), in place on p / state.  t = 1-based optimizer step."""
+                   l1_coefficient: float = 0.0, use_ghost_grads: bool = False, dead_feature_window: int = 5000,
+                   topk_idx: Optional[torch.Tensor] = None, topk_val: Optional[torch.Tensor] = None):
+    """One reference train_step (train_sae.py:278-411), in place on p / state.  t = 1-based optimizer step.
+    ``topk_idx`` / ``topk_val``: see sae_forward."""
     p["W_dec"] /= torch.norm(p["W_dec"], dim=1, keepdim=True)             # :307 set_decoder_norm_to_unit_norm
     dead_mask = (since_fired > dead_feature_window) if (use_ghost_grads and since_fired is not None) else None   # train_sae.py:330-332
-    fwd = sae_forward(p, x, k, mode, act=act, l1_coefficient=l1_coefficient, dead_mask=dead_mask)
+    fwd = sae_forward(p, x, k, mode, act=act, l1_coefficient=l1_coefficient, dead_mask=dead_mask, topk_idx=topk_idx, topk_val=topk_val)
     grads = sae_grads(p, x, fwd, mode, l1_coefficient=l1_coefficient, dead_mask=dead_mask)
     raw_grads = {n: g.clone() for n, g in grads.items()}
     acts = fwd["feature_acts"]

@@ -11,7 +11,8 @@ import numpy as np
 import pytest
 import torch
 
-from oracle.fused_topk_model import SEG, candidate_keys, f2ord, ord2f, select_row, tf32_trunc
+from oracle.fused_topk_model import (SEG, candidate_keys, candidate_keys_batch, f2ord, gather_threshold, ord2f, select_row, select_rows,
+                                      tf32_trunc)
 
 
 def _case(rows, d, F, seed, w_scale=None, worst_mantissa=False, offset=True):
@@ -109,3 +110,39 @@ def test_kept_keys_are_the_segment_maxima():
         others = np.delete(seg, cols)
         # a dropped column can only exceed a kept one inside one 128-ulp bucket (the low 7 bits were replaced by the column)
         assert np.all(f2ord(others).astype(np.int64) <= (f2ord(np.float32(kept_min)).astype(np.int64) | 127))
+
+
+@pytest.mark.parametrize("nseg", [1, 3, 20, 300, 800])
+def test_gather_threshold_keeps_the_quota(nseg):
+    """k_cand_select gathers the keys at or above tau, the smallest of the per-warp reports: at least min(96, nseg) keys, and tau
+    is one thread's best key (a segment maximum)."""
+    x, W, b = _case(4, 32, nseg * SEG, seed=nseg)
+    for keys in candidate_keys_batch(x, W, b, 8):
+        tau = gather_threshold(keys)
+        assert tau in set(keys[:, 0].tolist())
+        assert (keys >= tau).sum() >= min(96, nseg)
+        if nseg <= 32:                                 # every thread bids and every bid is reported: tau = the smallest maximum
+            assert tau == keys[:, 0].min()
+
+
+def test_u_below_and_the_early_stop_at_the_gathered_keys():
+    """Three segments (24 keys): the gathered set is always smaller than 128, so the rounds stop at G, and once every gathered key
+    is re-scored the bound on the rest is u_below, the best key under the threshold.  Both paths occur here, and every row is
+    still the exact top-k."""
+    rows, d, F, k = 64, 64, 3 * SEG, 4
+    x, W, b = _case(rows, d, F, seed=11)
+    keys = candidate_keys_batch(x, W, b, 8)
+    res = select_rows(x, W, b, k, keys=keys, c_keep=8, m_cand=k)
+    for a, kr, r in zip(x, keys, res):
+        exact = W.astype(np.float64) @ a.astype(np.float64) + b.astype(np.float64)
+        assert r["G"] == (kr >= r["tau"]).sum() < 128
+        assert r["rescored"] <= r["G"]
+        if not r["proven"]:
+            assert r["rescored"] == r["G"], "an unproven row re-scores until its gathered keys run out, not until 128"
+        else:
+            assert r["outside_max"] < r["tau_k"]
+        if r["u_src"] == "below":
+            assert r["rescored"] == r["G"] and r["u_below"] == kr[kr < r["tau"]].max()
+        assert np.array_equal(r["idx"], np.lexsort((np.arange(F), -exact))[:k])
+    assert any(r["proven"] and r["u_src"] == "below" for r in res), "no row proven on u_below"
+    assert any(r["rounds"] > 1 and r["rescored"] == r["G"] for r in res), "no row stopped early at the gathered keys"
