@@ -2,7 +2,8 @@
 
 The per-row kernels of the step (k_sae_prep, k_sae_decode, k_sae_grads, k_sae_grads_long, k_sae_adam_bulk / k_sae_adam_rows) hold
 a d_in row as CHUNKS float4 per lane, CHUNKS in {1, 2, 4, 6, 8, 12} for d_in up to 128, 256, 512, 768, 1024, 1536 (chunks_for in
-csrc/sae.cu).  The widths below take every instance, full and with idle lanes in the last chunk, on both encoder routes:
+csrc/sae_optim.cuh; both Adam kernels run its sae_adam_feature).  The widths below take every instance, full and with idle lanes
+in the last chunk, on both encoder routes:
 
   * fused: tf32 candidate GEMM + exact re-scoring, Adam in the bulk-copy pipeline (its ring depth varies with d) or, below
     d = 64, in the rows kernel;

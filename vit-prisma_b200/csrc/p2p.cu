@@ -18,6 +18,7 @@
 // The gradient is the SUM over ranks: each rank's local gradient already carries the 1/(global tokens) factor of the
 // mean loss, and the batch statistics the loss needs (column mean of x, sae.py:145) are reduced across ranks first.
 #include "common.cuh"
+#include "sae_optim.cuh"
 
 #define PB_MAX_RANKS 8
 
@@ -232,37 +233,46 @@ __global__ void k_p2p_publish_norm(P2PTables t, float* part_accum) {
   if (r < t.world) t.norm_parts[r][t.rank] = *part_accum;     // peer store
 }
 
-struct SaeScalarsP2P { float loss_sum, gnorm_sq, clip_coef, mse, l0, pos_count, grad_norm, reserved; };
-
-// after the norm barrier: total norm, clip coefficient, global loss statistics
-__global__ void k_p2p_finalize(P2PTables t, SaeScalarsP2P* sc, float max_norm, float inv_elems_global, float inv_rows_global) {
+// after the norm barrier: total norm, clip coefficient, global loss statistics (mse / l0: this rank's share of the global
+// mean, the ranks' shares add up)
+__global__ void k_p2p_finalize(P2PTables t, SaeScalars* sc, float max_norm, float inv_elems_global, float inv_rows_global) {
   float tot = 0.f;
   for (int r = 0; r < t.world; ++r) tot += t.norm_parts[t.rank][r];
-  const float norm = sqrtf(tot);
-  sc->gnorm_sq = tot;
-  sc->grad_norm = norm;
-  sc->clip_coef = max_norm > 0.f ? fminf(1.f, max_norm / (norm + 1e-6f)) : 1.f;
-  sc->mse = sc->loss_sum * inv_elems_global;      // this rank's share of the global mean (ranks' shares add up)
-  sc->l0 = sc->pos_count * inv_rows_global;
+  sae_publish_scalars(sc, tot, max_norm, inv_elems_global, inv_rows_global);
 }
 
 // ------------------------------------------------------------------------------------------- Adam on owned rows + all-gather
-struct AdamHyperP2P { float lr, beta1, beta2, eps, bc1, bc2_sqrt; };
-__device__ __forceinline__ float adam_upd(float p, float gr, float& m, float& v, const AdamHyperP2P& h) {   // same arithmetic as sae.cu adam_update
-  m = h.beta1 * m + (1.f - h.beta1) * gr;
-  v = h.beta2 * v + (1.f - h.beta2) * gr * gr;
-  float sq, rc;
-  asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(sq) : "f"(v));
-  const float denom = fmaf(sq, __frcp_rn(h.bc2_sqrt), h.eps);
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(rc) : "f"(denom));
-  return fmaf(-(h.lr * __frcp_rn(h.bc1)) * m, rc, p);
-}
+// the updated owned rows: own copy only (W_dec deferred to pb_p2p_push_dec), one multicast store, or stores to every rank's copy
+// (destination j = rank (rank + j) % world: every GPU addresses a different peer at a time, permutation traffic through the switch)
+struct AdamPeerOut {
+  float* const (&wdec_rot)[PB_MAX_RANKS];
+  float* const (&wenc_rot)[PB_MAX_RANKS];
+  float* const (&wlo_rot)[PB_MAX_RANKS];
+  float *own_dec, *mc_W_dec, *mc_W_encT;
+  int world, defer_dec;
+  int64_t base;
+  __device__ __forceinline__ void dec(int c4, const float (&w)[4]) const {
+    if (defer_dec) st4(own_dec + base + 4 * c4, w);                                                         // own copy only
+    else if (mc_W_dec) mc_st4(mc_W_dec + base + 4 * c4, w);                                                 // all-gather: one multicast store
+    else for (int j = 0; j < world; ++j) st4(wdec_rot[j] + base + 4 * c4, w);                              // all-gather: peer stores, own copy first
+  }
+  __device__ __forceinline__ void enc(int c4, const float (&p)[4], const float (&lo)[4]) const {
+    if (mc_W_encT) {
+      mc_st4(mc_W_encT + base + 4 * c4, p);
+    } else {
+      for (int j = 0; j < world; ++j) {
+        st4(wenc_rot[j] + base + 4 * c4, p);
+        if (wlo_rot[j]) st4(wlo_rot[j] + base + 4 * c4, lo);   // tf32 residual plane: dense 3xTF32 encoder only
+      }
+    }
+  }
+};
 
 template <int CHUNKS>
 __global__ void __launch_bounds__(256) k_p2p_adam_allgather(P2PTables t, int f0, int f1, int d, const float* __restrict__ gb_enc_red,
                                                            float* __restrict__ m_dec, float* __restrict__ v_dec, float* __restrict__ m_enc,
                                                            float* __restrict__ v_enc, float* __restrict__ m_be, float* __restrict__ v_be,
-                                                           const SaeScalarsP2P* __restrict__ sc, AdamHyperP2P h, float* __restrict__ mc_W_dec,
+                                                           const SaeScalars* __restrict__ sc, AdamHyper h, float* __restrict__ mc_W_dec,
                                                            float* __restrict__ mc_W_encT, float* __restrict__ mc_b_enc, float* __restrict__ wmax_accum,
                                                            int defer_dec) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
@@ -273,7 +283,6 @@ __global__ void __launch_bounds__(256) k_p2p_adam_allgather(P2PTables t, int f0,
   float* W_encT = t.W_encT[t.rank];
   const float* gWd = t.gW_dec[t.rank];
   const float* gWe = t.gW_encT[t.rank];
-  // destination j = rank (t.rank + j) % world: every GPU addresses a different peer at a time (permutation traffic through the switch)
   float *wdec_rot[PB_MAX_RANKS], *wenc_rot[PB_MAX_RANKS], *wlo_rot[PB_MAX_RANKS];
 #pragma unroll
   for (int j = 0; j < PB_MAX_RANKS; ++j) {
@@ -282,85 +291,15 @@ __global__ void __launch_bounds__(256) k_p2p_adam_allgather(P2PTables t, int f0,
   }
   for (int f = f0 + blockIdx.x * nw + warp; f < f1; f += gridDim.x * nw) {
     const int64_t base = (int64_t)f * d;
-    float w[CHUNKS][4], gq[CHUNKS][4];
-    float par = 0.f;
-#pragma unroll
-    for (int i = 0; i < CHUNKS; ++i) {
-      const int c4 = i * 32 + lane;
-      if (c4 < nvec) {
-        ld4(W_dec + base + 4 * c4, w[i]);
-        ld4(gWd + base + 4 * c4, gq[i]);
-#pragma unroll
-        for (int q = 0; q < 4; ++q) { gq[i][q] *= clip; par = fmaf(gq[i][q], w[i][q], par); }
-      } else {
-        w[i][0] = w[i][1] = w[i][2] = w[i][3] = gq[i][0] = gq[i][1] = gq[i][2] = gq[i][3] = 0.f;
-      }
-    }
-    par = warp_sum(par);
-    float nsq = 0.f;
-#pragma unroll
-    for (int i = 0; i < CHUNKS; ++i) {
-      const int c4 = i * 32 + lane;
-      if (c4 < nvec) {
-        float mm[4], vv[4];
-        ld4(m_dec + base + 4 * c4, mm);
-        ld4(v_dec + base + 4 * c4, vv);
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          w[i][q] = adam_upd(w[i][q], gq[i][q] - par * w[i][q], mm[q], vv[q], h);
-          nsq += w[i][q] * w[i][q];
-        }
-        st4(m_dec + base + 4 * c4, mm);
-        st4(v_dec + base + 4 * c4, vv);
-      }
-    }
-    const float inv_nrm = 1.f / sqrtf(warp_sum(nsq));
-#pragma unroll
-    for (int i = 0; i < CHUNKS; ++i) {
-      const int c4 = i * 32 + lane;
-      if (c4 < nvec) {
-#pragma unroll
-        for (int q = 0; q < 4; ++q) w[i][q] = w[i][q] * inv_nrm;
-        if (defer_dec) st4(W_dec + base + 4 * c4, w[i]);                                   // own copy only: pb_p2p_push_dec sends it later
-        else if (mc_W_dec) mc_st4(mc_W_dec + base + 4 * c4, w[i]);                         // all-gather: one multicast store
-        else for (int j = 0; j < t.world; ++j) st4(wdec_rot[j] + base + 4 * c4, w[i]);     // all-gather: peer stores, own copy first
-      }
-    }
-    float esq = 0.f, elo = 0.f;
-#pragma unroll
-    for (int i = 0; i < CHUNKS; ++i) {
-      const int c4 = i * 32 + lane;
-      if (c4 < nvec) {
-        float p[4], gr[4], mm[4], vv[4], lo[4];
-        ld4(W_encT + base + 4 * c4, p);
-        ld4(gWe + base + 4 * c4, gr);
-        ld4(m_enc + base + 4 * c4, mm);
-        ld4(v_enc + base + 4 * c4, vv);
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          p[q] = adam_upd(p[q], gr[q] * clip, mm[q], vv[q], h);
-          lo[q] = tf32_lo(p[q]);
-          esq = fmaf(p[q], p[q], esq);
-          const float tl = p[q] - tf32_trunc(p[q]);
-          elo = fmaf(tl, tl, elo);
-        }
-        st4(m_enc + base + 4 * c4, mm);
-        st4(v_enc + base + 4 * c4, vv);
-        if (mc_W_encT) {
-          mc_st4(mc_W_encT + base + 4 * c4, p);
-        } else {
-          for (int j = 0; j < t.world; ++j) {
-            st4(wenc_rot[j] + base + 4 * c4, p);
-            if (wlo_rot[j]) st4(wlo_rot[j] + base + 4 * c4, lo);             // tf32 residual plane: dense 3xTF32 encoder only
-          }
-        }
-      }
-    }
+    float esq, elo;
+    sae_adam_feature<CHUNKS>(W_dec + base, gWd + base, m_dec + base, v_dec + base, W_encT + base, gWe + base, m_enc + base, v_enc + base,
+                             clip, h, nvec, true,
+                             AdamPeerOut{wdec_rot, wenc_rot, wlo_rot, W_dec, mc_W_dec, mc_W_encT, t.world, defer_dec, base}, esq, elo);
     enc_best = fmaxf(enc_best, warp_sum(esq));
     enc_best_lo = fmaxf(enc_best_lo, warp_sum(elo));
     if (lane == 0) {
       float mm = m_be[f], vv = v_be[f];
-      const float nb = adam_upd(t.b_enc[t.rank][f], gb_enc_red[f] * clip, mm, vv, h);
+      const float nb = adam_update(t.b_enc[t.rank][f], gb_enc_red[f] * clip, mm, vv, h);
       m_be[f] = mm;
       v_be[f] = vv;
       if (mc_b_enc) mc_st1(mc_b_enc + f, nb);
@@ -390,21 +329,20 @@ __global__ void __launch_bounds__(256) k_p2p_small_updates(P2PTables t, const fl
                                                           const float* __restrict__ gb_dec_red, float* __restrict__ m_bd,
                                                           float* __restrict__ v_bd, const float* __restrict__ fired_red,
                                                           float* __restrict__ since_fired, float* __restrict__ act_freq,
-                                                          const SaeScalarsP2P* __restrict__ sc, AdamHyperP2P h, int d, int F) {
+                                                          const SaeScalars* __restrict__ sc, AdamHyper h, int d, int F) {
   if (blockIdx.x == 0 && threadIdx.x < t.world) {      // publish this rank's encoder row-norm maxima to every peer (was its own launch)
     t.norm_parts[threadIdx.x][PB_MAX_RANKS + t.rank] = wmax_accum[0];
     t.norm_parts[threadIdx.x][2 * PB_MAX_RANKS + t.rank] = wmax_accum[1];
   }
   const float clip = sc->clip_coef;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < F; i += gridDim.x * blockDim.x) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < max(F, d); i += gridDim.x * blockDim.x) {   // d_sae may be below d_in
     if (i < d) {
       float mm = m_bd[i], vv = v_bd[i];
-      b_dec[i] = adam_upd(b_dec[i], gb_dec_red[i] * clip, mm, vv, h);
+      b_dec[i] = adam_update(b_dec[i], gb_dec_red[i] * clip, mm, vv, h);
       m_bd[i] = mm;
       v_bd[i] = vv;
     }
-    if (since_fired) since_fired[i] = fired_red[i] > 0.f ? 0.f : since_fired[i] + 1.f;
-    if (act_freq) act_freq[i] += fired_red[i];
+    if (i < F) dead_feature_counters(since_fired, act_freq, i, fired_red[i], since_fired ? since_fired[i] : 0.f, act_freq ? act_freq[i] : 0.f);
   }
 }
 
@@ -469,30 +407,20 @@ extern "C" int pb_p2p_adam_allgather(const PbP2PStep* s, pb_stream_t stream) {
   PB_CHECK_ARG(s->step >= 1, "pb_p2p_adam_allgather: step counter starts at 1");
   cudaStream_t st = (cudaStream_t)stream;
   const int per = s->F / s->world, f0 = s->rank * per, f1 = f0 + per;
-  AdamHyperP2P h;
-  h.lr = s->lr; h.beta1 = s->beta1; h.beta2 = s->beta2; h.eps = s->adam_eps;
-  h.bc1 = 1.f - powf(s->beta1, (float)s->step);
-  h.bc2_sqrt = sqrtf(1.f - powf(s->beta2, (float)s->step));
-  k_p2p_finalize<<<1, 1, 0, st>>>(t, (SaeScalarsP2P*)s->scalars, s->max_grad_norm, 1.f / ((float)s->global_rows * (float)s->d),
+  const AdamHyper h = adam_hyper(s->lr, s->beta1, s->beta2, s->adam_eps, s->step);
+  k_p2p_finalize<<<1, 1, 0, st>>>(t, (SaeScalars*)s->scalars, s->max_grad_norm, 1.f / ((float)s->global_rows * (float)s->d),
                                   1.f / (float)s->global_rows);
   PB_LAUNCH_CHECK();
   const int d = s->d;
   int grid = pb_sm_count() * 4;
   if (grid > (per + 7) / 8) grid = (per + 7) / 8;
   PB_CHECK_ARG((!s->mc_W_dec == !s->mc_W_encT) && (!s->mc_W_dec == !s->mc_b_enc), "pb_p2p_adam_allgather: all three multicast parameter views or none");
-#define PB_P2P_ADAM(CH) k_p2p_adam_allgather<CH><<<grid, 256, 0, st>>>(t, f0, f1, d, s->gb_enc_red, s->m_dec, s->v_dec, s->m_enc, s->v_enc, s->m_be, s->v_be, (const SaeScalarsP2P*)s->scalars, h, s->mc_W_dec, s->mc_W_encT, s->mc_b_enc, s->part_accum + 1, s->defer_dec)
-  const int nvec = d / 4;
-  if (d % 4 != 0 || nvec > 384) { pb_set_error("pb_p2p_adam_allgather: d_in=%d unsupported", d); return PB_EUNSUPPORTED; }
-  if (nvec <= 32) PB_P2P_ADAM(1);
-  else if (nvec <= 64) PB_P2P_ADAM(2);
-  else if (nvec <= 128) PB_P2P_ADAM(4);
-  else if (nvec <= 192) PB_P2P_ADAM(6);
-  else if (nvec <= 256) PB_P2P_ADAM(8);
-  else PB_P2P_ADAM(12);
-#undef PB_P2P_ADAM
+  PB_DISPATCH_CHUNKS(chunks_for(d), (k_p2p_adam_allgather<C_><<<grid, 256, 0, st>>>(t, f0, f1, d, s->gb_enc_red, s->m_dec, s->v_dec, s->m_enc,
+                                     s->v_enc, s->m_be, s->v_be, (const SaeScalars*)s->scalars, h, s->mc_W_dec, s->mc_W_encT, s->mc_b_enc,
+                                     s->part_accum + 1, s->defer_dec)));
   PB_LAUNCH_CHECK();
-  k_p2p_small_updates<<<(s->F + 255) / 256, 256, 0, st>>>(t, s->part_accum + 1, s->b_dec, s->gb_dec_red, s->m_bd, s->v_bd, s->fired_red, s->since_fired,
-                                                        s->act_freq, (const SaeScalarsP2P*)s->scalars, h, d, s->F);
+  k_p2p_small_updates<<<((s->F > d ? s->F : d) + 255) / 256, 256, 0, st>>>(t, s->part_accum + 1, s->b_dec, s->gb_dec_red, s->m_bd, s->v_bd, s->fired_red, s->since_fired,
+                                                        s->act_freq, (const SaeScalars*)s->scalars, h, d, s->F);
   PB_LAUNCH_CHECK();
   return PB_OK;
 }

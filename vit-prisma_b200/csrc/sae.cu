@@ -14,21 +14,8 @@
 //        fused clip + decoder-parallel-gradient removal + Adam + decoder row renorm + dead-feature counters.
 // No host synchronisation anywhere: scalars (loss, norm, clip coefficient) live in a device struct.
 #include "common.cuh"
-#include <stdlib.h>
 #include "tc_common.cuh"
-
-// ---------------------------------------------------------------------------------------------
-// device scalars of one step
-struct SaeScalars {
-  float loss_sum;      // sum_b sum_c (out-x)^2 / nf[b]            (mse = loss_sum / (Bt*d))
-  float gnorm_sq;      // sum of squares of all gradient entries (pre-clip)
-  float clip_coef;     // min(1, max_norm / (norm + 1e-6))
-  float mse;           // loss_sum / (Bt*d)
-  float l0;            // mean number of positive activations per token
-  float pos_count;     // accumulator for l0
-  float grad_norm;     // sqrt(gnorm_sq)
-  float reserved;
-};
+#include "sae_optim.cuh"
 
 // ---------------------------------------------------------------------------------------------
 // 1. prep: run-time input normalisation + decoder-bias subtraction (sae.py:78-87, 557-566)
@@ -708,35 +695,21 @@ __global__ void __launch_bounds__(256) k_sae_finalize(const float* __restrict__ 
   if (threadIdx.x == 0) {
     float t = sc->gnorm_sq;
     for (int i = 0; i < 8; ++i) t += red[i];
-    const float norm = sqrtf(t);
-    sc->gnorm_sq = t;
-    sc->grad_norm = norm;
-    sc->clip_coef = max_norm > 0.f ? fminf(1.f, max_norm / (norm + 1e-6f)) : 1.f;
-    sc->mse = sc->loss_sum * inv_elems;
-    sc->l0 = sc->pos_count * inv_rows;
+    sae_publish_scalars(sc, t, max_norm, inv_elems, inv_rows);
   }
 }
 
 // ---------------------------------------------------------------------------------------------
-// 7. optimizer: clip -> remove decoder-parallel gradient -> Adam -> unit-norm decoder rows (+ counters)
-//    (train_sae.py:394-401, sae.py:275-297, torch.optim.Adam defaults betas (0.9, 0.999), eps 1e-8, no weight decay)
-//    The row renorm is the *next* step's set_decoder_norm_to_unit_norm() (train_sae.py:307) applied early; forward
-//    and backward of every later step see identical numbers.
-struct AdamHyper { float lr, beta1, beta2, eps, bc1, bc2_sqrt; };  // bc1 = 1-beta1^t, bc2_sqrt = sqrt(1-beta2^t)
-
-// torch.optim.Adam (single tensor, no amsgrad / weight decay): m, v exactly as torch computes them; the parameter update
-// -(lr / bc1) m / (sqrt(v) / bc2_sqrt + eps) uses MUFU sqrt / reciprocal approximations (relative error ~1e-7 of an update that is
-// itself ~lr relative to the parameter: 1e-10 on the parameter, against a 1e-4 parity bar).  The IEEE sqrt + two divisions of the
-// first version were ~30 of the ~45 instructions per element and made the optimizer issue-bound.
-__device__ __forceinline__ float adam_update(float p, float gr, float& m, float& v, const AdamHyper& h) {
-  m = h.beta1 * m + (1.f - h.beta1) * gr;
-  v = h.beta2 * v + (1.f - h.beta2) * gr * gr;
-  float sq, rc;
-  asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(sq) : "f"(v));
-  const float denom = fmaf(sq, __frcp_rn(h.bc2_sqrt), h.eps);
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(rc) : "f"(denom));
-  return fmaf(-(h.lr * __frcp_rn(h.bc1)) * m, rc, p);
-}
+// 7. optimizer (sae_optim.cuh): one warp per feature, rows in registers, updated rows stored back in place
+struct AdamRowsOut {
+  float *W_dec, *W_encT, *W_encT_lo;
+  int64_t base;
+  __device__ __forceinline__ void dec(int c4, const float (&w)[4]) const { st4(W_dec + base + 4 * c4, w); }
+  __device__ __forceinline__ void enc(int c4, const float (&p)[4], const float (&lo)[4]) const {
+    st4(W_encT + base + 4 * c4, p);
+    if (W_encT_lo) st4(W_encT_lo + base + 4 * c4, lo);
+  }
+};
 
 template <int CHUNKS>
 __global__ void __launch_bounds__(256) k_sae_adam_rows(float* __restrict__ W_dec, float* __restrict__ W_encT, float* __restrict__ W_encT_lo,
@@ -753,86 +726,16 @@ __global__ void __launch_bounds__(256) k_sae_adam_rows(float* __restrict__ W_dec
   float enc_best = 0.f, enc_best_lo = 0.f;
   for (int f = blockIdx.x * nw + warp; f < F; f += gridDim.x * nw) {
     const int64_t base = (int64_t)f * d;
-    // ---- decoder row
-    float w[CHUNKS][4], gq[CHUNKS][4];
-    float par = 0.f;
-#pragma unroll
-    for (int i = 0; i < CHUNKS; ++i) {
-      const int c4 = i * 32 + lane;
-      if (c4 < nvec) {
-        ld4(W_dec + base + 4 * c4, w[i]);
-        ld4(gW_dec + base + 4 * c4, gq[i]);
-#pragma unroll
-        for (int q = 0; q < 4; ++q) { gq[i][q] *= clip; par = fmaf(gq[i][q], w[i][q], par); }
-      } else {
-        w[i][0] = w[i][1] = w[i][2] = w[i][3] = gq[i][0] = gq[i][1] = gq[i][2] = gq[i][3] = 0.f;
-      }
-    }
-    par = warp_sum(par);
-    float nsq = 0.f;
-#pragma unroll
-    for (int i = 0; i < CHUNKS; ++i) {
-      const int c4 = i * 32 + lane;
-      if (c4 < nvec) {
-        float mm[4], vv[4];
-        ld4(m_dec + base + 4 * c4, mm);
-        ld4(v_dec + base + 4 * c4, vv);
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const float gr = gq[i][q] - par * w[i][q];
-          w[i][q] = adam_update(w[i][q], gr, mm[q], vv[q], h);
-          nsq += w[i][q] * w[i][q];
-        }
-        st4(m_dec + base + 4 * c4, mm);
-        st4(v_dec + base + 4 * c4, vv);
-      }
-    }
-    const float inv_nrm = 1.f / sqrtf(warp_sum(nsq));
-#pragma unroll
-    for (int i = 0; i < CHUNKS; ++i) {
-      const int c4 = i * 32 + lane;
-      if (c4 < nvec) {
-        if (renorm) {
-#pragma unroll
-          for (int q = 0; q < 4; ++q) w[i][q] = w[i][q] * inv_nrm;
-        }
-        st4(W_dec + base + 4 * c4, w[i]);
-      }
-    }
-    // ---- encoder row (feature-major)
-    float esq = 0.f, elo = 0.f;
-#pragma unroll
-    for (int i = 0; i < CHUNKS; ++i) {
-      const int c4 = i * 32 + lane;
-      if (c4 < nvec) {
-        float p[4], gr[4], mm[4], vv[4], lo[4];
-        ld4(W_encT + base + 4 * c4, p);
-        ld4(gW_encT + base + 4 * c4, gr);
-        ld4(m_enc + base + 4 * c4, mm);
-        ld4(v_enc + base + 4 * c4, vv);
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          p[q] = adam_update(p[q], gr[q] * clip, mm[q], vv[q], h);
-          lo[q] = tf32_lo(p[q]);
-          esq = fmaf(p[q], p[q], esq);
-          const float tl = p[q] - tf32_trunc(p[q]);
-          elo = fmaf(tl, tl, elo);
-        }
-        st4(W_encT + base + 4 * c4, p);
-        st4(m_enc + base + 4 * c4, mm);
-        st4(v_enc + base + 4 * c4, vv);
-        if (W_encT_lo) st4(W_encT_lo + base + 4 * c4, lo);
-      }
-    }
+    float esq, elo;
+    sae_adam_feature<CHUNKS>(W_dec + base, gW_dec + base, m_dec + base, v_dec + base, W_encT + base, gW_encT + base, m_enc + base,
+                             v_enc + base, clip, h, nvec, renorm, AdamRowsOut{W_dec, W_encT, W_encT_lo, base}, esq, elo);
     if (enc_norm_max) { enc_best = fmaxf(enc_best, warp_sum(esq)); enc_best_lo = fmaxf(enc_best_lo, warp_sum(elo)); }
     if (lane == 0) {
       float mm = m_be[f], vv = v_be[f];
       b_enc[f] = adam_update(b_enc[f], gb_enc[f] * clip, mm, vv, h);
       m_be[f] = mm;
       v_be[f] = vv;
-      // dead-feature bookkeeping (train_sae.py:356-361)
-      if (since_fired) since_fired[f] = fired[f] > 0.f ? 0.f : since_fired[f] + 1.f;
-      if (act_freq) act_freq[f] += fired[f];
+      dead_feature_counters(since_fired, act_freq, f, fired[f], since_fired ? since_fired[f] : 0.f, act_freq ? act_freq[f] : 0.f);
     }
   }
   // largest encoder-column norm after the update (error bound of the fused encoder's tf32 pass); norms are >= 0 so the
@@ -855,6 +758,13 @@ __global__ void __launch_bounds__(256) k_sae_adam_rows(float* __restrict__ W_dec
 // another warp was still updating -- the first 12-warp version deadlocked in run r2d.)
 constexpr int AB_MAX_STAGES = 12;
 constexpr int AB_THREADS = 32 * (1 + AB_MAX_STAGES);
+
+// a consumer warp updates its ring slot in place: W_dec at st[0, d), W_encT at st[4d, 5d)
+struct AdamSlotOut {
+  float *wd, *we;
+  __device__ __forceinline__ void dec(int c4, const float (&w)[4]) const { st4(wd + 4 * c4, w); }
+  __device__ __forceinline__ void enc(int c4, const float (&p)[4], const float (&)[4]) const { st4(we + 4 * c4, p); }
+};
 
 __device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src), "r"(bytes), "r"(bar)
@@ -935,76 +845,9 @@ k_sae_adam_bulk(float* __restrict__ W_dec, float* __restrict__ W_encT, float* __
     }
     mbar_wait(full_bar(s), ph);
     float* st = data_generic + (size_t)s * 8 * d;
-    float *wd = st, *gd = st + d, *md = st + 2 * d, *vd = st + 3 * d, *we = st + 4 * d, *ge = st + 5 * d, *me = st + 6 * d, *ve = st + 7 * d;
-    // ---- decoder row: clip, remove the component parallel to the (unit-norm) row, Adam, renormalise
-    float w[CHUNKS][4], gq[CHUNKS][4];
-    float par = 0.f;
-#pragma unroll
-    for (int c = 0; c < CHUNKS; ++c) {
-      const int c4 = c * 32 + lane;
-      if (c4 < nvec) {
-        ld4(wd + 4 * c4, w[c]);
-        ld4(gd + 4 * c4, gq[c]);
-#pragma unroll
-        for (int q = 0; q < 4; ++q) { gq[c][q] *= clip; par = fmaf(gq[c][q], w[c][q], par); }
-      } else {
-        w[c][0] = w[c][1] = w[c][2] = w[c][3] = gq[c][0] = gq[c][1] = gq[c][2] = gq[c][3] = 0.f;
-      }
-    }
-    par = warp_sum(par);
-    float nsq = 0.f;
-#pragma unroll
-    for (int c = 0; c < CHUNKS; ++c) {
-      const int c4 = c * 32 + lane;
-      if (c4 < nvec) {
-        float mm[4], vv[4];
-        ld4(md + 4 * c4, mm);
-        ld4(vd + 4 * c4, vv);
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const float gr = gq[c][q] - par * w[c][q];
-          w[c][q] = adam_update(w[c][q], gr, mm[q], vv[q], h);
-          nsq += w[c][q] * w[c][q];
-        }
-        st4(md + 4 * c4, mm);
-        st4(vd + 4 * c4, vv);
-      }
-    }
-    const float inv_nrm = 1.f / sqrtf(warp_sum(nsq));
-#pragma unroll
-    for (int c = 0; c < CHUNKS; ++c) {
-      const int c4 = c * 32 + lane;
-      if (c4 < nvec) {
-        if (renorm) {
-#pragma unroll
-          for (int q = 0; q < 4; ++q) w[c][q] = w[c][q] * inv_nrm;
-        }
-        st4(wd + 4 * c4, w[c]);
-      }
-    }
-    // ---- encoder row
-    float esq = 0.f, elo = 0.f;
-#pragma unroll
-    for (int c = 0; c < CHUNKS; ++c) {
-      const int c4 = c * 32 + lane;
-      if (c4 < nvec) {
-        float p[4], gr[4], mm[4], vv[4];
-        ld4(we + 4 * c4, p);
-        ld4(ge + 4 * c4, gr);
-        ld4(me + 4 * c4, mm);
-        ld4(ve + 4 * c4, vv);
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          p[q] = adam_update(p[q], gr[q] * clip, mm[q], vv[q], h);
-          esq = fmaf(p[q], p[q], esq);
-          const float tl = p[q] - tf32_trunc(p[q]);
-          elo = fmaf(tl, tl, elo);
-        }
-        st4(we + 4 * c4, p);
-        st4(me + 4 * c4, mm);
-        st4(ve + 4 * c4, vv);
-      }
-    }
+    float esq, elo;
+    sae_adam_feature<CHUNKS>(st, st + d, st + 2 * d, st + 3 * d, st + 4 * d, st + 5 * d, st + 6 * d, st + 7 * d, clip, h, nvec, renorm,
+                             AdamSlotOut{st, st + 4 * d}, esq, elo);
     enc_best = fmaxf(enc_best, warp_sum(esq));
     enc_best_lo = fmaxf(enc_best_lo, warp_sum(elo));
     __syncwarp();
@@ -1023,8 +866,7 @@ k_sae_adam_bulk(float* __restrict__ W_dec, float* __restrict__ W_encT, float* __
       b_enc[f] = adam_update(be, gbe * clip, mbe, vbe, h);
       m_be[f] = mbe;
       v_be[f] = vbe;
-      if (since_fired) since_fired[f] = fr > 0.f ? 0.f : sf + 1.f;
-      if (act_freq) act_freq[f] = af + fr;
+      dead_feature_counters(since_fired, act_freq, f, fr, sf, af);
       asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // the ring slot has been read: hand it back
       mbar_arrive(empty_bar(s));
     }
@@ -1082,28 +924,6 @@ __global__ void __launch_bounds__(256) k_unit_rows(float* __restrict__ W, float*
 // =============================================================================================
 // host side
 // =============================================================================================
-static int chunks_for(int d) {
-  if (d % 4 != 0) return -1;
-  const int nvec = d / 4;
-  if (nvec <= 32) return 1;
-  if (nvec <= 64) return 2;
-  if (nvec <= 128) return 4;
-  if (nvec <= 192) return 6;
-  if (nvec <= 256) return 8;
-  if (nvec <= 384) return 12;
-  return -1;
-}
-#define PB_DISPATCH_CHUNKS(CH, CALL)                                                   \
-  switch (CH) {                                                                        \
-    case 1: { constexpr int C_ = 1; CALL; } break;                                     \
-    case 2: { constexpr int C_ = 2; CALL; } break;                                     \
-    case 4: { constexpr int C_ = 4; CALL; } break;                                     \
-    case 6: { constexpr int C_ = 6; CALL; } break;                                     \
-    case 8: { constexpr int C_ = 8; CALL; } break;                                     \
-    case 12: { constexpr int C_ = 12; CALL; } break;                                   \
-    default: pb_set_error("sae: d_in=%d unsupported (needs d %% 4 == 0 and d <= 1536)", d); return PB_EUNSUPPORTED; \
-  }
-
 static int persistent_grid(int warps_per_cta, int items) {
   int ctas = pb_sm_count() * 4;
   const int need = (items + warps_per_cta - 1) / warps_per_cta;
@@ -1287,15 +1107,10 @@ extern "C" int pb_sae_adam(const PbSaeStep* s, pb_stream_t stream) {
   PB_CHECK_ARG(s->step >= 1, "pb_sae_adam: step counter starts at 1");
   cudaStream_t st = (cudaStream_t)stream;
   const int d = s->d, F = s->F, ch = chunks_for(d);
-  AdamHyper h;
-  h.lr = s->lr; h.beta1 = s->beta1; h.beta2 = s->beta2; h.eps = s->adam_eps;
-  h.bc1 = 1.f - powf(s->beta1, (float)s->step);
-  h.bc2_sqrt = sqrtf(1.f - powf(s->beta2, (float)s->step));
+  const AdamHyper h = adam_hyper(s->lr, s->beta1, s->beta2, s->adam_eps, s->step);
   const int grid = persistent_grid(8, F);
   if (s->enc_norm_max) PB_CUDA(cudaMemsetAsync(s->enc_norm_max, 0, 2 * sizeof(float), st));
-  static int bulk_mode = -1;        // PB_SAE_ADAM=rows forces the register kernel (A/B measurements)
-  if (bulk_mode < 0) { const char* e = getenv("PB_SAE_ADAM"); bulk_mode = (e && !strcmp(e, "rows")) ? 0 : 1; }
-  if (bulk_mode && !s->W_encT_lo && d % 4 == 0 && d >= 64) {      // no tf32 residual plane to maintain: the bulk-copy pipeline
+  if (!s->W_encT_lo && d >= 64) {      // no tf32 residual plane to maintain: the bulk-copy pipeline
     const size_t stage = (size_t)8 * d * 4;
     int S = (int)((200 * 1024) / stage);
     if (S > 12) S = 12;
@@ -1303,24 +1118,13 @@ extern "C" int pb_sae_adam(const PbSaeStep* s, pb_stream_t stream) {
       const size_t smem = 256 + (size_t)S * stage;
       int g2 = pb_sm_count();
       if (g2 > F) g2 = F;
-#define PB_ADAM_BULK(CH)                                                                                                              \
-  do {                                                                                                                                \
-    auto kern = k_sae_adam_bulk<CH>;                                                                                                  \
-    PB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));                                     \
-    PB_LAUNCH_PDL(kern, g2, 32 * (1 + S), smem, st, s->W_dec, s->W_encT, s->b_enc, s->gW_dec, s->gW_encT, s->gb_enc, s->m_dec, s->v_dec, s->m_enc, \
-                  s->v_enc, s->m_be, s->v_be, s->fired, s->since_fired, s->act_freq, (const SaeScalars*)s->scalars,                    \
-                  h, F, d, s->renorm_decoder, s->enc_norm_max, S, s->b_dec, s->gb_dec, s->m_bd, s->v_bd);                               \
-  } while (0)
-      switch (ch) {
-        case 1: PB_ADAM_BULK(1); break;
-        case 2: PB_ADAM_BULK(2); break;
-        case 4: PB_ADAM_BULK(4); break;
-        case 6: PB_ADAM_BULK(6); break;
-        case 8: PB_ADAM_BULK(8); break;
-        case 12: PB_ADAM_BULK(12); break;
-        default: pb_set_error("sae: d_in=%d unsupported", d); return PB_EUNSUPPORTED;
-      }
-#undef PB_ADAM_BULK
+      PB_DISPATCH_CHUNKS(ch, {
+        auto kern = k_sae_adam_bulk<C_>;
+        PB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        PB_LAUNCH_PDL(kern, g2, 32 * (1 + S), smem, st, s->W_dec, s->W_encT, s->b_enc, s->gW_dec, s->gW_encT, s->gb_enc, s->m_dec, s->v_dec,
+                      s->m_enc, s->v_enc, s->m_be, s->v_be, s->fired, s->since_fired, s->act_freq, (const SaeScalars*)s->scalars, h, F, d,
+                      s->renorm_decoder, s->enc_norm_max, S, s->b_dec, s->gb_dec, s->m_bd, s->v_bd);
+      });
       return PB_OK;
     }
   }
@@ -1330,6 +1134,17 @@ extern "C" int pb_sae_adam(const PbSaeStep* s, pb_stream_t stream) {
                                                                      F, d, s->renorm_decoder, s->enc_norm_max)));
   PB_LAUNCH_CHECK();
   k_sae_adam_vec<<<(d + 255) / 256, 256, 0, st>>>(s->b_dec, s->gb_dec, s->m_bd, s->v_bd, (const SaeScalars*)s->scalars, h, d);
+  PB_LAUNCH_CHECK();
+  return PB_OK;
+}
+
+// Adam on a flat parameter vector with the step's clip coefficient (the extra parameters of the Gated SAE and the Transcoder)
+extern "C" int pb_adam_vec(float* p, const float* g, float* m, float* v, int32_t n, const void* scalars, float lr, float beta1, float beta2,
+                           float eps, int32_t step, pb_stream_t stream) {
+  PB_CHECK_ARG(p && g && m && v && scalars && n >= 0 && step >= 1, "pb_adam_vec: bad arguments");
+  if (n == 0) return PB_OK;
+  const int grid = (n + 255) / 256 < pb_sm_count() * 8 ? (n + 255) / 256 : pb_sm_count() * 8;
+  k_sae_adam_vec<<<grid, 256, 0, (cudaStream_t)stream>>>(p, g, m, v, (const SaeScalars*)scalars, adam_hyper(lr, beta1, beta2, eps, step), n);
   PB_LAUNCH_CHECK();
   return PB_OK;
 }

@@ -10,12 +10,9 @@
 #include <algorithm>
 
 #include "common.cuh"
+#include "sae_optim.cuh"
 
 namespace {
-
-struct SaeScalars {   // same layout as sae.cu (8 floats)
-  float loss_sum, gnorm_sq, clip_coef, mse, l0, pos_count, grad_norm, reserved;
-};
 
 // ---- out[c][r] = in[r][c] (+ tf32 residual plane of the transposed values)
 __global__ void __launch_bounds__(256) k_transpose32(const float* __restrict__ in, float* __restrict__ out, float* __restrict__ out_lo, int rows,
@@ -155,11 +152,7 @@ __global__ void __launch_bounds__(256) k_sumsq(const float* __restrict__ a, int6
   }
 }
 __global__ void k_grad_finish(SaeScalars* sc, float max_norm, float inv_elems, float inv_rows) {
-  const float norm = sqrtf(sc->gnorm_sq);
-  sc->grad_norm = norm;
-  sc->clip_coef = max_norm > 0.f ? fminf(1.f, max_norm / (norm + 1e-6f)) : 1.f;   // clip_grad_norm_ (train_sae.py:394-397)
-  sc->mse = sc->loss_sum * inv_elems;
-  sc->l0 = sc->pos_count * inv_rows;
+  sae_publish_scalars(sc, sc->gnorm_sq, max_norm, inv_elems, inv_rows);
 }
 
 // ---- ghost grads ------------------------------------------------------------------------------------------------
@@ -488,19 +481,6 @@ __global__ void __launch_bounds__(256) k_gated_l1_rows(float* __restrict__ gW_de
   if (lane == 0 && cs != 0.f) atomicAdd(l1_sum, cs * wn);
 }
 
-struct AdamVecHyper { float lr, beta1, beta2, eps, bc1, bc2_sqrt; };
-__global__ void __launch_bounds__(256) k_adam_vec(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
-                                                  const SaeScalars* __restrict__ sc, AdamVecHyper h, int n) {
-  const float clip = sc->clip_coef;
-  for (int i = blockIdx.x * 256 + threadIdx.x; i < n; i += gridDim.x * 256) {
-    const float gr = g[i] * clip;
-    const float mm = h.beta1 * m[i] + (1.f - h.beta1) * gr;
-    const float vv = h.beta2 * v[i] + (1.f - h.beta2) * gr * gr;
-    m[i] = mm; v[i] = vv;
-    p[i] -= (h.lr / h.bc1) * (mm / (sqrtf(vv) / h.bc2_sqrt + h.eps));
-  }
-}
-
 inline void col_grid(int rows, int F, dim3& grid, int& rpc) {
   const int gx = (F + 255) / 256;
   const int chunks = std::max(1, std::min(rows, (pb_sm_count() * 8 + gx - 1) / gx));
@@ -578,19 +558,6 @@ extern "C" int pb_sumsq(const float* a, int64_t n, float* acc, pb_stream_t strea
 extern "C" int pb_sae_clip_finish(void* scalars, float max_grad_norm, int32_t rows, int32_t d, pb_stream_t stream) {
   PB_CHECK_ARG(scalars && rows > 0 && d > 0, "pb_sae_clip_finish: bad arguments");
   k_grad_finish<<<1, 1, 0, (cudaStream_t)stream>>>((SaeScalars*)scalars, max_grad_norm, 1.f / ((float)rows * (float)d), 1.f / (float)rows);
-  PB_LAUNCH_CHECK();
-  return PB_OK;
-}
-
-extern "C" int pb_adam_vec(float* p, const float* g, float* m, float* v, int32_t n, const void* scalars, float lr, float beta1, float beta2,
-                           float eps, int32_t step, pb_stream_t stream) {
-  PB_CHECK_ARG(p && g && m && v && scalars && n >= 0 && step >= 1, "pb_adam_vec: bad arguments");
-  if (n == 0) return PB_OK;
-  AdamVecHyper h;
-  h.lr = lr; h.beta1 = beta1; h.beta2 = beta2; h.eps = eps;
-  h.bc1 = 1.f - powf(beta1, (float)step);
-  h.bc2_sqrt = sqrtf(1.f - powf(beta2, (float)step));
-  k_adam_vec<<<std::min((n + 255) / 256, pb_sm_count() * 8), 256, 0, (cudaStream_t)stream>>>(p, g, m, v, (const SaeScalars*)scalars, h, n);
   PB_LAUNCH_CHECK();
   return PB_OK;
 }

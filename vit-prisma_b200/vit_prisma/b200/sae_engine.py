@@ -66,6 +66,9 @@ L.register_signatures({
     "pb_sae_fused_workspace": (i32, [i32, i32, i32, C.POINTER(i64), C.POINTER(i64)]),
     "pb_sae_encode_topk_fused": (i32, [C.POINTER(PbSaeEncode), vp]),
     "pb_rownorm_max": (i32, [vp, i32, i32, vp, vp]),
+    "pb_sumsq": (i32, [vp, i64, vp, vp]),
+    "pb_sae_clip_finish": (i32, [vp, f32, i32, i32, vp]),
+    "pb_adam_vec": (i32, [vp, vp, vp, vp, i32, vp, f32, f32, f32, f32, i32, vp]),
 })
 
 NORM_MODE = {"none": 0, None: 0, "layer_norm": 1, "constant_norm_rescale": 2}
@@ -322,8 +325,24 @@ class SaeStepEngine:
     def _optimizer_stages(self, s: PbSaeStep, x: torch.Tensor, lr: float, since_fired, act_freq):
         """(name, callable, info) of the stages after backward; the data-parallel engine replaces them with its peer-memory phases."""
         lib, st = L.get_lib(), _stream()
+        kernel = "k_sae_adam_rows" if self.W_encT_lo is not None or self.d < 64 else "k_sae_adam_bulk"   # pb_sae_adam's choice
         return [("adam (clip + decoder-parallel-gradient removal + Adam + row renorm)", lambda: L.check(lib.pb_sae_adam(C.byref(s), st)),
-                 dict(bytes=60 * self.d * self.F, ncu=r"k_sae_adam_rows"))]
+                 dict(bytes=60 * self.d * self.F, ncu=kernel))]
+
+    def _clip_and_adam(self, x: torch.Tensor, lr: float, since_fired, act_freq, grads, extra) -> None:
+        """Optimizer tail of the engines whose gradients come from dense products: global norm over ``grads`` -> clip coefficient,
+        ``pb_sae_adam`` on the SAE parameters, then ``pb_adam_vec`` on each ``(param, grad, m, v)`` of ``extra``."""
+        lib, st = L.get_lib(), _stream()
+        self.scalars[1:2].zero_()
+        acc = self.scalars[1:].data_ptr()
+        for t in grads:
+            L.check(lib.pb_sumsq(t.data_ptr(), t.numel(), acc, st), "pb_sumsq")
+        L.check(lib.pb_sae_clip_finish(self.scalars.data_ptr(), self.max_grad_norm, x.shape[0], self.d, st), "pb_sae_clip_finish")
+        s = self._desc(x, training=True, lr=lr, since_fired=since_fired, act_freq=act_freq, want_out=False)
+        L.check(lib.pb_sae_adam(C.byref(s), st), "pb_sae_adam")
+        for p, g, m, v in extra:
+            L.check(lib.pb_adam_vec(p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), p.numel(), self.scalars.data_ptr(), lr, self.betas[0],
+                                    self.betas[1], self.adam_eps, self.step_count, st), "pb_adam_vec")
 
     @torch.no_grad()
     def time_stages(self, x: torch.Tensor, lr: float, since_fired=None, act_freq=None, reps: int = 5) -> dict:

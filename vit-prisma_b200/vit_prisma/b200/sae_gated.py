@@ -24,7 +24,7 @@ from . import ops
 from .sae_dense import _gemm_impl, _p, colsum, gemm32, gemv_rows, transpose
 from .sae_engine import SaeStepEngine, _need_cuda, _stream
 
-i32, i64, f32, vp = C.c_int32, C.c_int64, C.c_float, C.c_void_p
+i32, f32, vp = C.c_int32, C.c_float, C.c_void_p
 
 L.register_signatures({
     "pb_gated_fwd": (i32, [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, vp]),
@@ -32,9 +32,6 @@ L.register_signatures({
     "pb_gated_bwd": (i32, [vp, vp, vp, vp, vp, vp, vp, vp, f32, vp, vp, vp, vp, i32, i32, vp]),
     "pb_row_norms": (i32, [vp, vp, i32, i32, vp]),
     "pb_gated_l1_rows": (i32, [vp, vp, vp, vp, f32, vp, i32, i32, vp]),
-    "pb_sumsq": (i32, [vp, i64, vp, vp]),
-    "pb_sae_clip_finish": (i32, [vp, f32, i32, i32, vp]),
-    "pb_adam_vec": (i32, [vp, vp, vp, vp, i32, vp, f32, f32, f32, f32, i32, vp]),
 })
 
 
@@ -144,17 +141,9 @@ class SaeGatedStepEngine(SaeStepEngine):
         L.check(sc(self.gb_dec.data_ptr(), self._zero_idx.data_ptr(), 1, d, colsum(ga).data_ptr(), 2.0, st), "pb_scatter_add_rows")
         L.check(sc(self.gb_dec.data_ptr(), self._zero_idx.data_ptr(), 1, d, gemv_rows(self.W_encT, self.dsum).data_ptr(), -1.0, st),
                 "pb_scatter_add_rows")
-        # global norm over the six trained tensors -> clip coefficient
-        self.scalars[1:2].zero_()
-        acc = self.scalars[1:].data_ptr()
-        for t in (self.gW_dec, self.gW_encT, self.gb_enc, self.gb_dec, self.gr_mag, self.gb_mag):
-            L.check(lib.pb_sumsq(t.data_ptr(), t.numel(), acc, st), "pb_sumsq")
-        L.check(lib.pb_sae_clip_finish(self.scalars.data_ptr(), self.max_grad_norm, rows, d, st), "pb_sae_clip_finish")
-        s = self._desc(x, training=True, lr=lr, since_fired=since_fired, act_freq=act_freq, want_out=False)
-        L.check(lib.pb_sae_adam(C.byref(s), st), "pb_sae_adam")
-        for p, g, m, v in ((self.r_mag, self.gr_mag, self.m_r, self.v_r), (self.b_mag, self.gb_mag, self.m_bm, self.v_bm)):
-            L.check(lib.pb_adam_vec(p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), F, self.scalars.data_ptr(), lr, self.betas[0],
-                                    self.betas[1], self.adam_eps, self.step_count, st), "pb_adam_vec")
+        # global norm over the six trained tensors -> clip coefficient -> Adam
+        self._clip_and_adam(x, lr, since_fired, act_freq, (self.gW_dec, self.gW_encT, self.gb_enc, self.gb_dec, self.gr_mag, self.gb_mag),
+                            ((self.r_mag, self.gr_mag, self.m_r, self.v_r), (self.b_mag, self.gb_mag, self.m_bm, self.v_bm)))
         return self.scalars
 
     def loss_terms(self, rows: int) -> dict:

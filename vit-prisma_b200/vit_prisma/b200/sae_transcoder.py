@@ -14,7 +14,6 @@ b_dec; ``pb_adam_vec`` updates W_skip and b_dec_out with the same clip coefficie
 """
 from __future__ import annotations
 
-import ctypes as C
 from typing import Optional
 
 import torch
@@ -24,12 +23,6 @@ from . import ops
 from .sae_dense import SaeDenseStepEngine, _gemm_impl, _p, colsum, gemm32, gemv_rows, transpose
 from .sae_engine import _need_cuda, _stream, topk_dense
 
-i32, f32, vp = C.c_int32, C.c_float, C.c_void_p
-L.register_signatures({
-    "pb_sumsq": (i32, [vp, C.c_int64, vp, vp]),
-    "pb_sae_clip_finish": (i32, [vp, f32, i32, i32, vp]),
-    "pb_adam_vec": (i32, [vp, vp, vp, vp, i32, vp, f32, f32, f32, f32, i32, vp]),
-})
 
 
 class SaeTranscoderStepEngine(SaeDenseStepEngine):
@@ -111,7 +104,7 @@ class SaeTranscoderStepEngine(SaeDenseStepEngine):
 
     def _train_step_tc(self, x, y, lr, since_fired, act_freq, want_out) -> torch.Tensor:
         lib, st = L.get_lib(), _stream()
-        rows, d, F = x.shape[0], self.d, self.F
+        rows, d = x.shape[0], self.d
         self.step_count += 1
         acts = self._forward(x, y, want_out, training=True)
         l1_grad = (self.l1_coefficient / rows) if self.activation != "topk" else 0.0       # TopK: no sparsity term (transcoder.py:96-100)
@@ -131,23 +124,13 @@ class SaeTranscoderStepEngine(SaeDenseStepEngine):
         self.gb_dec.zero_()
         L.check(lib.pb_scatter_add_rows(self.gb_dec.data_ptr(), self._zero_idx.data_ptr(), 1, d, tmp.data_ptr(), -1.0, st), "pb_scatter_add_rows")
         grads = [self.gW_dec, self.gW_encT, self.gb_enc, self.gb_dec, self.gb_dec_out]
+        extra = [(self.b_dec_out, self.gb_dec_out, self.m_bo, self.v_bo)]
         if self.W_skip is not None:
             xT, xT_lo = transpose(x)                                         # [d, rows]
             gemm32(gT, gT_lo, xT, xT_lo, out0=self.gW_skip)                  # gW_skip = g^T @ x   ([d_out, d_in], out += x @ W_skip^T)
             grads.append(self.gW_skip)
-        self.scalars[1:2].zero_()
-        acc = self.scalars[1:].data_ptr()
-        for t in grads:
-            L.check(lib.pb_sumsq(t.data_ptr(), t.numel(), acc, st), "pb_sumsq")
-        L.check(lib.pb_sae_clip_finish(self.scalars.data_ptr(), self.max_grad_norm, rows, d, st), "pb_sae_clip_finish")
-        s = self._desc(x, training=True, lr=lr, since_fired=since_fired, act_freq=act_freq, want_out=False)
-        L.check(lib.pb_sae_adam(C.byref(s), st), "pb_sae_adam")
-        extra = [(self.b_dec_out, self.gb_dec_out, self.m_bo, self.v_bo)]
-        if self.W_skip is not None:
             extra.append((self.W_skip, self.gW_skip, self.m_sk, self.v_sk))
-        for p, g, m, v in extra:
-            L.check(lib.pb_adam_vec(p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), p.numel(), self.scalars.data_ptr(), lr, self.betas[0],
-                                    self.betas[1], self.adam_eps, self.step_count, st), "pb_adam_vec")
+        self._clip_and_adam(x, lr, since_fired, act_freq, grads, extra)
         return self.scalars
 
     def loss_terms(self, rows: int) -> dict:
