@@ -33,7 +33,7 @@ typedef struct CUstream_st* pb_stream_t; /* == cudaStream_t */
 #endif
 
 enum { PB_OK = 0, PB_EINVAL = -1, PB_ECUDA = -2, PB_EUNSUPPORTED = -3, PB_ENODEVICE = -4 };
-enum { PB_F32 = 0, PB_BF16 = 1 };
+enum { PB_F32 = 0, PB_BF16 = 1, PB_F16 = 2 /* tensor maps of the fused SAE encoder's fp16 operand copies only */ };
 /* activation_name of HookedViTConfig (models/layers/mlp.py:41-62, models/activation_fns.py:19-58) */
 enum { PB_ACT_NONE = 0, PB_ACT_RELU = 1, PB_ACT_GELU = 2, PB_ACT_SILU = 3, PB_ACT_GELU_NEW = 4,
        PB_ACT_GELU_FAST = 5, PB_ACT_QUICK_GELU = 6, PB_ACT_TANH_RELU = 7, PB_ACT_EXP = 8 };
@@ -238,11 +238,19 @@ typedef struct {
   float* enc_norm_max;
   /* 1: pb_sae_step_reset already zeroed gcol / gbdec2 / the work header for this step (pb_sae_backward then skips its memsets) */
   int32_t pre_zeroed;
+  /* fp16 operand copy of W_encT [F][d] for the fused encoder's fp16 candidate GEMM, rewritten by pb_sae_adam (fp16 rounding
+   * of each updated row, clamped to +-65504; needs d % 8 == 0), and [1] max_f ||W_encT[f,:] - fp16(W_encT[f,:])||_2 after the
+   * update.  Both NULL: no copy is kept.                                                                                  */
+  void* W_encT16; float* enc16_lo_max;
 } PbSaeStep;
 
 /* sae_in = norm_in(x) - b_dec (+ tf32 residual, row mean / std, column sums of x) -- sae.py:78-87, 557-566 */
 PB_API int pb_sae_prep(const float* x, const float* b_dec, float* sae_in, float* sae_in_lo, float* mu, float* sd,
                        float* xsum, int32_t rows, int32_t d, int32_t norm_mode, pb_stream_t stream);
+/* pb_sae_prep that also writes sae_in16 [rows][d], the fp16 rounding of sae_in clamped to +-65504 (the A operand of the fused
+ * encoder's fp16 candidate GEMM); sae_in16 may be NULL                                                                     */
+PB_API int pb_sae_prep16(const float* x, const float* b_dec, float* sae_in, void* sae_in16, float* mu, float* sd,
+                         float* xsum, int32_t rows, int32_t d, int32_t norm_mode, pb_stream_t stream);
 /* torch.topk(hidden_pre, k, dim=-1) (sae.py:803-805): idx int32 / val fp32 [rows][k], sorted by value descending,
  * ties broken towards the lower index; feat_count[f] += 1 per selection (may be NULL);
  * scratch >= rows * ceil(F / 24576) * k * 8 bytes when F > 24576, else unused.                     */
@@ -291,11 +299,18 @@ typedef struct {
   int32_t* fb_count;            /* [2]: rows that took the exact path in this call; candidates re-scored over the other rows */
   int32_t* fb_rows;             /* [rows]                                                                                 */
   float* fb_scratch; int64_t fb_scratch_bytes;   /* >= F * 4 bytes; one d_sae row per resident CTA of the exact path      */
+  /* fp16 candidate GEMM (all three set, d % 8 == 0): phase 1 reads these fp16 copies of sae_in / W_encT (pb_sae_prep16,
+   * pb_f16_copy / pb_sae_adam) instead of the fp32 operands, and phase 2 bounds the error with the fp16 residuals:
+   * ||a - fp16(a)|| (from sae_in) and enc16_lo_max [1] = max_f ||W_encT[f,:] - fp16(W_encT[f,:])||.  NULL: the tf32 GEMM.    */
+  const void* sae_in16; const void* W_encT16; const float* enc16_lo_max;
 } PbSaeEncode;
 PB_API int pb_sae_fused_workspace(int32_t rows, int32_t F, int32_t c_keep, int64_t* cand_bytes, int64_t* fb_scratch_bytes);
 PB_API int pb_sae_encode_topk_fused(const PbSaeEncode* e, pb_stream_t stream);
 /* out[0] = max_f ||W[f,:]||_2, out[1] = max_f ||W[f,:] - tf32_trunc(W[f,:])||_2 over the rows of a contiguous fp32 [F][d] matrix */
 PB_API int pb_rownorm_max(const float* W, int32_t F, int32_t d, float* out, pb_stream_t stream);
+/* W16 = fp16(W) (round to nearest, clamped to +-65504) for a contiguous fp32 [rows][d] matrix, d % 4 == 0, and, when lo_max is
+ * not NULL, lo_max[0] = max_r ||W[r,:] - W16[r,:]||_2                                                                        */
+PB_API int pb_f16_copy(const float* W, int64_t rows, int32_t d, void* W16, float* lo_max, pb_stream_t stream);
 
 /* ------------------------------------------------ dense SAE step pieces (activation_fn_str = "relu" + L1) and ghost grads
  * StandardSparseAutoencoder.forward with a dense activation executes six [tokens x d_sae x d_in] products

@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <string.h>
@@ -95,6 +96,22 @@ __device__ __forceinline__ float tf32_lo(float x) {
   uint32_t r;
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x - tf32_trunc(x)));
   return __uint_as_float(r);
+}
+
+// fp16 operand copy of the fused SAE encoder: round to nearest, clamped to the largest finite fp16 (NaN -> -65504), so that no Inf
+// or NaN reaches the GEMM; the clamped part shows up in the residual norm and widens the error bound instead
+__device__ __forceinline__ float f16_sat(float x) { return __half2float(__float2half_rn(fminf(fmaxf(x, -65504.f), 65504.f))); }
+// four values -> their fp16 copies packed in 8 bytes; rsq += sum of the squared residuals x - fp16(x) (each exact in fp32)
+__device__ __forceinline__ uint2 f16x4(const float (&v)[4], float& rsq) {
+  float h[4];
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    h[q] = f16_sat(v[q]);
+    const float r = v[q] - h[q];
+    rsq = fmaf(r, r, rsq);
+  }
+  const __half2 a = __floats2half2_rn(h[0], h[1]), b = __floats2half2_rn(h[2], h[3]);   // exact: h[] are fp16 values
+  return make_uint2(*reinterpret_cast<const uint32_t*>(&a), *reinterpret_cast<const uint32_t*>(&b));
 }
 
 // ------------------------------------------------------------- activations

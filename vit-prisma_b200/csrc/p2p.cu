@@ -256,7 +256,7 @@ struct AdamPeerOut {
     else if (mc_W_dec) mc_st4(mc_W_dec + base + 4 * c4, w);                                                 // all-gather: one multicast store
     else for (int j = 0; j < world; ++j) st4(wdec_rot[j] + base + 4 * c4, w);                              // all-gather: peer stores, own copy first
   }
-  __device__ __forceinline__ void enc(int c4, const float (&p)[4], const float (&lo)[4]) const {
+  __device__ __forceinline__ void enc(int c4, const float (&p)[4], const float (&lo)[4], uint2) const {   // no fp16 copy on this path
     if (mc_W_encT) {
       mc_st4(mc_W_encT + base + 4 * c4, p);
     } else {
@@ -291,10 +291,10 @@ __global__ void __launch_bounds__(256) k_p2p_adam_allgather(P2PTables t, int f0,
   }
   for (int f = f0 + blockIdx.x * nw + warp; f < f1; f += gridDim.x * nw) {
     const int64_t base = (int64_t)f * d;
-    float esq, elo;
+    float esq, elo, e16;
     sae_adam_feature<CHUNKS>(W_dec + base, gWd + base, m_dec + base, v_dec + base, W_encT + base, gWe + base, m_enc + base, v_enc + base,
                              clip, h, nvec, true,
-                             AdamPeerOut{wdec_rot, wenc_rot, wlo_rot, W_dec, mc_W_dec, mc_W_encT, t.world, defer_dec, base}, esq, elo);
+                             AdamPeerOut{wdec_rot, wenc_rot, wlo_rot, W_dec, mc_W_dec, mc_W_encT, t.world, defer_dec, base}, esq, elo, e16);
     enc_best = fmaxf(enc_best, warp_sum(esq));
     enc_best_lo = fmaxf(enc_best_lo, warp_sum(elo));
     if (lane == 0) {

@@ -20,13 +20,14 @@
 // ---------------------------------------------------------------------------------------------
 // 1. prep: run-time input normalisation + decoder-bias subtraction (sae.py:78-87, 557-566)
 //    layer_norm mode: mu = mean(x); xc = x - mu; std = unbiased std(xc); xn = xc / (std + 1e-5)
-//    sae_in = xn - b_dec ;  sae_in_lo = tf32 residual (A operand of the 3xTF32 encoder GEMM)
+//    sae_in = xn - b_dec ;  sae_in_lo = tf32 residual (A operand of the 3xTF32 encoder GEMM);
+//    sae_in16 = fp16 copy (A operand of the fused encoder's fp16 candidate GEMM)
 //    xsum[c] += x[b,c]  (batch mean for _compute_mse_loss's centring, sae.py:145)
 // one warp per token row; row kept in registers.
 template <int CHUNKS>
 __global__ void __launch_bounds__(256) k_sae_prep(const float* __restrict__ x, const float* __restrict__ b_dec, float* __restrict__ sae_in,
-                                                  float* __restrict__ sae_in_lo, float* __restrict__ mu_out, float* __restrict__ std_out,
-                                                  int rows, int d, int norm_mode, float eps) {
+                                                  float* __restrict__ sae_in_lo, __half* __restrict__ sae_in16, float* __restrict__ mu_out,
+                                                  float* __restrict__ std_out, int rows, int d, int norm_mode, float eps) {
   pb_pdl();
   const int lane = threadIdx.x & 31;
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -82,6 +83,10 @@ __global__ void __launch_bounds__(256) k_sae_prep(const float* __restrict__ x, c
       (void)inv;
       st4(sae_in + (int64_t)row * d + 4 * c4, o);
       if (sae_in_lo) st4(sae_in_lo + (int64_t)row * d + 4 * c4, lo);
+      if (sae_in16) {
+        float unused = 0.f;
+        *reinterpret_cast<uint2*>(sae_in16 + (int64_t)row * d + 4 * c4) = f16x4(o, unused);
+      }
     }
   }
 }
@@ -703,16 +708,24 @@ __global__ void __launch_bounds__(256) k_sae_finalize(const float* __restrict__ 
 // 7. optimizer (sae_optim.cuh): one warp per feature, rows in registers, updated rows stored back in place
 struct AdamRowsOut {
   float *W_dec, *W_encT, *W_encT_lo;
+  __half* W_encT16;
   int64_t base;
   __device__ __forceinline__ void dec(int c4, const float (&w)[4]) const { st4(W_dec + base + 4 * c4, w); }
-  __device__ __forceinline__ void enc(int c4, const float (&p)[4], const float (&lo)[4]) const {
+  __device__ __forceinline__ void enc(int c4, const float (&p)[4], const float (&lo)[4], uint2 p16) const {
     st4(W_encT + base + 4 * c4, p);
     if (W_encT_lo) st4(W_encT_lo + base + 4 * c4, lo);
+    if (W_encT16) *reinterpret_cast<uint2*>(W_encT16 + base + 4 * c4) = p16;
   }
 };
 
+// max_f of the per-feature norms (atomic max on the bit patterns: norms are >= 0, so the bit pattern orders like the value)
+__device__ __forceinline__ void atomic_max_norm(float* out, float best_sq) {
+  if (best_sq > 0.f) atomicMax(reinterpret_cast<unsigned int*>(out), __float_as_uint(sqrtf(best_sq)));
+}
+
 template <int CHUNKS>
 __global__ void __launch_bounds__(256) k_sae_adam_rows(float* __restrict__ W_dec, float* __restrict__ W_encT, float* __restrict__ W_encT_lo,
+                                                       __half* __restrict__ W_encT16, float* __restrict__ enc16_lo_max,
                                                        float* __restrict__ b_enc, const float* __restrict__ gW_dec,
                                                        const float* __restrict__ gW_encT, const float* __restrict__ gb_enc,
                                                        float* __restrict__ m_dec, float* __restrict__ v_dec, float* __restrict__ m_enc,
@@ -723,13 +736,14 @@ __global__ void __launch_bounds__(256) k_sae_adam_rows(float* __restrict__ W_dec
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
   const int nvec = d >> 2;
   const float clip = sc->clip_coef;
-  float enc_best = 0.f, enc_best_lo = 0.f;
+  float enc_best = 0.f, enc_best_lo = 0.f, enc_best16 = 0.f;
   for (int f = blockIdx.x * nw + warp; f < F; f += gridDim.x * nw) {
     const int64_t base = (int64_t)f * d;
-    float esq, elo;
+    float esq, elo, e16;
     sae_adam_feature<CHUNKS>(W_dec + base, gW_dec + base, m_dec + base, v_dec + base, W_encT + base, gW_encT + base, m_enc + base,
-                             v_enc + base, clip, h, nvec, renorm, AdamRowsOut{W_dec, W_encT, W_encT_lo, base}, esq, elo);
+                             v_enc + base, clip, h, nvec, renorm, AdamRowsOut{W_dec, W_encT, W_encT_lo, W_encT16, base}, esq, elo, e16);
     if (enc_norm_max) { enc_best = fmaxf(enc_best, warp_sum(esq)); enc_best_lo = fmaxf(enc_best_lo, warp_sum(elo)); }
+    if (enc16_lo_max) enc_best16 = fmaxf(enc_best16, warp_sum(e16));
     if (lane == 0) {
       float mm = m_be[f], vv = v_be[f];
       b_enc[f] = adam_update(b_enc[f], gb_enc[f] * clip, mm, vv, h);
@@ -744,6 +758,7 @@ __global__ void __launch_bounds__(256) k_sae_adam_rows(float* __restrict__ W_dec
     atomicMax(reinterpret_cast<unsigned int*>(enc_norm_max), __float_as_uint(sqrtf(enc_best)));
     atomicMax(reinterpret_cast<unsigned int*>(enc_norm_max) + 1, __float_as_uint(sqrtf(enc_best_lo)));
   }
+  if (enc16_lo_max && lane == 0) atomic_max_norm(enc16_lo_max, enc_best16);
 }
 
 // ---- 7b. the same update as a bulk-copy pipeline ---------------------------------------------------------------------
@@ -759,11 +774,16 @@ __global__ void __launch_bounds__(256) k_sae_adam_rows(float* __restrict__ W_dec
 constexpr int AB_MAX_STAGES = 12;
 constexpr int AB_THREADS = 32 * (1 + AB_MAX_STAGES);
 
-// a consumer warp updates its ring slot in place: W_dec at st[0, d), W_encT at st[4d, 5d)
+// a consumer warp updates its ring slot in place: W_dec at st[0, d), W_encT at st[4d, 5d), and the fp16 copy of W_encT in the
+// first half of the gW_dec row st[d, 2d), which the decoder update has consumed before the encoder row starts
 struct AdamSlotOut {
   float *wd, *we;
+  __half* we16;
   __device__ __forceinline__ void dec(int c4, const float (&w)[4]) const { st4(wd + 4 * c4, w); }
-  __device__ __forceinline__ void enc(int c4, const float (&p)[4], const float (&)[4]) const { st4(we + 4 * c4, p); }
+  __device__ __forceinline__ void enc(int c4, const float (&p)[4], const float (&)[4], uint2 p16) const {
+    st4(we + 4 * c4, p);
+    if (we16) *reinterpret_cast<uint2*>(we16 + 4 * c4) = p16;
+  }
 };
 
 __device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
@@ -781,7 +801,8 @@ k_sae_adam_bulk(float* __restrict__ W_dec, float* __restrict__ W_encT, float* __
                 float* __restrict__ m_enc, float* __restrict__ v_enc, float* __restrict__ m_be, float* __restrict__ v_be,
                 const float* __restrict__ fired, float* __restrict__ since_fired, float* __restrict__ act_freq,
                 const SaeScalars* __restrict__ sc, AdamHyper h, int F, int d, int renorm, float* __restrict__ enc_norm_max, int S,
-                float* __restrict__ b_dec, const float* __restrict__ gb_dec, float* __restrict__ m_bd, float* __restrict__ v_bd) {
+                float* __restrict__ b_dec, const float* __restrict__ gb_dec, float* __restrict__ m_bd, float* __restrict__ v_bd,
+                __half* __restrict__ W_encT16, float* __restrict__ enc16_lo_max) {
   pb_pdl_trigger();
   extern __shared__ __align__(128) unsigned char ab_smem[];
   const uint32_t s0 = smem_u32(ab_smem);
@@ -830,7 +851,7 @@ k_sae_adam_bulk(float* __restrict__ W_dec, float* __restrict__ W_encT, float* __
   }
   const int nvec = d >> 2;
   const float clip = sc->clip_coef;
-  float enc_best = 0.f, enc_best_lo = 0.f;
+  float enc_best = 0.f, enc_best_lo = 0.f, enc_best16 = 0.f;
   for (int i = warp - 1; i < n_mine; i += S) {
     const int s = i % S;
     const uint32_t ph = (uint32_t)(i / S) & 1u;
@@ -845,11 +866,12 @@ k_sae_adam_bulk(float* __restrict__ W_dec, float* __restrict__ W_encT, float* __
     }
     mbar_wait(full_bar(s), ph);
     float* st = data_generic + (size_t)s * 8 * d;
-    float esq, elo;
+    float esq, elo, e16;
     sae_adam_feature<CHUNKS>(st, st + d, st + 2 * d, st + 3 * d, st + 4 * d, st + 5 * d, st + 6 * d, st + 7 * d, clip, h, nvec, renorm,
-                             AdamSlotOut{st, st + 4 * d}, esq, elo);
+                             AdamSlotOut{st, st + 4 * d, W_encT16 ? reinterpret_cast<__half*>(st + d) : nullptr}, esq, elo, e16);
     enc_best = fmaxf(enc_best, warp_sum(esq));
     enc_best_lo = fmaxf(enc_best_lo, warp_sum(elo));
+    if (W_encT16) enc_best16 = fmaxf(enc_best16, warp_sum(e16));
     __syncwarp();
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // generic-proxy writes above -> visible to the bulk-copy engine
     __syncwarp();
@@ -861,6 +883,7 @@ k_sae_adam_bulk(float* __restrict__ W_dec, float* __restrict__ W_encT, float* __
       bulk_store(W_encT + base, src + 4 * row_bytes, row_bytes);
       bulk_store(m_enc + base, src + 6 * row_bytes, row_bytes);
       bulk_store(v_enc + base, src + 7 * row_bytes, row_bytes);
+      if (W_encT16) bulk_store(W_encT16 + base, src + 1 * row_bytes, row_bytes / 2);
       asm volatile("cp.async.bulk.commit_group;" ::: "memory");
       // bias + dead-feature bookkeeping (train_sae.py:356-361) while the stores drain
       b_enc[f] = adam_update(be, gbe * clip, mbe, vbe, h);
@@ -875,6 +898,7 @@ k_sae_adam_bulk(float* __restrict__ W_dec, float* __restrict__ W_encT, float* __
     atomicMax(reinterpret_cast<unsigned int*>(enc_norm_max), __float_as_uint(sqrtf(enc_best)));
     atomicMax(reinterpret_cast<unsigned int*>(enc_norm_max) + 1, __float_as_uint(sqrtf(enc_best_lo)));
   }
+  if (enc16_lo_max && lane == 0) atomic_max_norm(enc16_lo_max, enc_best16);
   asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
 }
 
@@ -931,14 +955,16 @@ static int persistent_grid(int warps_per_cta, int items) {
   return ctas < 1 ? 1 : ctas;
 }
 
-extern "C" int pb_sae_prep(const float* x, const float* b_dec, float* sae_in, float* sae_in_lo, float* mu, float* sd, float* xsum, int32_t rows,
-                           int32_t d, int32_t norm_mode, pb_stream_t stream) {
+static int launch_prep(const float* x, const float* b_dec, float* sae_in, float* sae_in_lo, __half* sae_in16, float* mu, float* sd, float* xsum,
+                       int32_t rows, int32_t d, int32_t norm_mode, pb_stream_t stream) {
   PB_CHECK_ARG(x && b_dec && sae_in && rows >= 0 && d > 0, "pb_sae_prep: bad arguments");
   PB_CHECK_ARG(norm_mode == 0 || (mu && sd), "pb_sae_prep: mu/std buffers required when normalising");
+  PB_CHECK_ARG(!sae_in16 || ((uintptr_t)sae_in16 & 7) == 0, "pb_sae_prep16: sae_in16 must be 8-byte aligned");
   if (rows == 0) return PB_OK;
   cudaStream_t st = (cudaStream_t)stream;
   const int ch = chunks_for(d);
-  PB_DISPATCH_CHUNKS(ch, PB_LAUNCH_PDL(k_sae_prep<C_>, (rows + 7) / 8, 256, 0, st, x, b_dec, sae_in, sae_in_lo, mu, sd, rows, d, norm_mode, 1e-5f));
+  PB_DISPATCH_CHUNKS(ch, PB_LAUNCH_PDL(k_sae_prep<C_>, (rows + 7) / 8, 256, 0, st, x, b_dec, sae_in, sae_in_lo, sae_in16, mu, sd, rows, d, norm_mode,
+                                       1e-5f));
   if (xsum) {
     PB_CUDA(cudaMemsetAsync(xsum, 0, sizeof(float) * d, st));
     const int rpc = 8;
@@ -946,6 +972,16 @@ extern "C" int pb_sae_prep(const float* x, const float* b_dec, float* sae_in, fl
     PB_LAUNCH_CHECK();
   }
   return PB_OK;
+}
+
+extern "C" int pb_sae_prep(const float* x, const float* b_dec, float* sae_in, float* sae_in_lo, float* mu, float* sd, float* xsum, int32_t rows,
+                           int32_t d, int32_t norm_mode, pb_stream_t stream) {
+  return launch_prep(x, b_dec, sae_in, sae_in_lo, nullptr, mu, sd, xsum, rows, d, norm_mode, stream);
+}
+
+extern "C" int pb_sae_prep16(const float* x, const float* b_dec, float* sae_in, void* sae_in16, float* mu, float* sd, float* xsum, int32_t rows,
+                             int32_t d, int32_t norm_mode, pb_stream_t stream) {
+  return launch_prep(x, b_dec, sae_in, nullptr, (__half*)sae_in16, mu, sd, xsum, rows, d, norm_mode, stream);
 }
 
 static int launch_topk(const float* vals, const int* map, int64_t row_stride, int F, int seg_len, int nseg, int k, int* oi, float* ov,
@@ -1109,7 +1145,11 @@ extern "C" int pb_sae_adam(const PbSaeStep* s, pb_stream_t stream) {
   const int d = s->d, F = s->F, ch = chunks_for(d);
   const AdamHyper h = adam_hyper(s->lr, s->beta1, s->beta2, s->adam_eps, s->step);
   const int grid = persistent_grid(8, F);
+  PB_CHECK_ARG(!s->W_encT16 == !s->enc16_lo_max, "pb_sae_adam: W_encT16 and enc16_lo_max go together");
+  PB_CHECK_ARG(!s->W_encT16 || (d % 8 == 0 && ((uintptr_t)s->W_encT16 & 15) == 0), "pb_sae_adam: the fp16 copy of W_encT needs d %% 8 == 0");
+  __half* const W16 = (__half*)s->W_encT16;
   if (s->enc_norm_max) PB_CUDA(cudaMemsetAsync(s->enc_norm_max, 0, 2 * sizeof(float), st));
+  if (s->enc16_lo_max) PB_CUDA(cudaMemsetAsync(s->enc16_lo_max, 0, sizeof(float), st));
   if (!s->W_encT_lo && d >= 64) {      // no tf32 residual plane to maintain: the bulk-copy pipeline
     const size_t stage = (size_t)8 * d * 4;
     int S = (int)((200 * 1024) / stage);
@@ -1123,12 +1163,13 @@ extern "C" int pb_sae_adam(const PbSaeStep* s, pb_stream_t stream) {
         PB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         PB_LAUNCH_PDL(kern, g2, 32 * (1 + S), smem, st, s->W_dec, s->W_encT, s->b_enc, s->gW_dec, s->gW_encT, s->gb_enc, s->m_dec, s->v_dec,
                       s->m_enc, s->v_enc, s->m_be, s->v_be, s->fired, s->since_fired, s->act_freq, (const SaeScalars*)s->scalars, h, F, d,
-                      s->renorm_decoder, s->enc_norm_max, S, s->b_dec, s->gb_dec, s->m_bd, s->v_bd);
+                      s->renorm_decoder, s->enc_norm_max, S, s->b_dec, s->gb_dec, s->m_bd, s->v_bd, W16, s->enc16_lo_max);
       });
       return PB_OK;
     }
   }
-  PB_DISPATCH_CHUNKS(ch, (k_sae_adam_rows<C_><<<grid, 256, 0, st>>>(s->W_dec, s->W_encT, s->W_encT_lo, s->b_enc, s->gW_dec, s->gW_encT, s->gb_enc,
+  PB_DISPATCH_CHUNKS(ch, (k_sae_adam_rows<C_><<<grid, 256, 0, st>>>(s->W_dec, s->W_encT, s->W_encT_lo, W16, s->enc16_lo_max, s->b_enc, s->gW_dec,
+                                                                     s->gW_encT, s->gb_enc,
                                                                      s->m_dec, s->v_dec, s->m_enc, s->v_enc, s->m_be, s->v_be, s->fired,
                                                                      s->since_fired, s->act_freq, (const SaeScalars*)s->scalars, h,
                                                                      F, d, s->renorm_decoder, s->enc_norm_max)));

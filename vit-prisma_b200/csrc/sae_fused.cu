@@ -2,10 +2,12 @@
 // written to HBM (reference sae/sae.py:557-581 `sae_in @ W_enc + b_enc` followed by TopK.forward :795-808 `torch.topk`).
 //
 // Approximate-then-rescore, exact by construction:
-//   1. k_enc_cand     persistent wgmma GEMM, ONE tf32 pass (the fp32 operands are read by the tensor core with their 13 low
-//                     mantissa bits ignored), 128 x 256 tiles: a tile's columns are two 128-feature segments.  The epilogue never
-//                     stores the tile: per segment, every thread turns the 32 values it holds of each of its two token rows into
-//                     packed keys (order-preserving int of the value, the low 7 bits replaced by the column inside the segment)
+//   1. k_enc_cand     persistent wgmma GEMM, ONE pass at 11 significant bits, 128 x 256 tiles: a tile's columns are two 128-feature
+//                     segments.  Either on the fp32 operands, read as tf32 (the tensor core ignores their 13 low mantissa bits), or
+//                     on fp16 copies of them (round to nearest, clamped to +-65504): the same precision at half the bytes.  The
+//                     GEMM is bound by the operand stream from L2 (3.6 GB per call at the bench shape in fp32), so the fp16 pass,
+//                     which also runs at twice the tensor rate, takes about half the time.  The epilogue never stores the tile:
+//                     per segment, every thread turns the 32 values it holds of each of its two token rows into packed keys (order-preserving int of the value, the low 7 bits replaced by the column inside the segment)
 //                     and keeps the 8 largest with sorting networks, the four threads sharing a row merge their lists by
 //                     shuffles, and one of them writes the first C_KEEP x 4 bytes.  Per token: d_sae / 128 segments x C_KEEP keys
 //                     (6 KB at d_sae = 24576) instead of a 98 KB dense row.
@@ -14,8 +16,9 @@
 //                     exact top-k of the re-scored values (ties -> lower index, sorted descending), and a proof that no
 //                     feature outside the candidate set can belong to the exact top-k:
 //                         ub(best key not selected, or last kept key of a segment whose keys were all selected) + E_row < tau_k
-//                     where E_row bounds |tf32 product - exact| by Cauchy-Schwarz: 2^-9 ||sae_in_row|| max_f ||W_enc[:, f]||
-//                     (each operand loses < 2^-10 relative to truncation).  Rows that fail the proof go on a list.
+//                     where E_row bounds |one-pass product - exact| by Cauchy-Schwarz on the operand residuals (a - read(a),
+//                     w - read(w); each < 2^-10 relative for tf32 truncation, 2^-11 for fp16 rounding) plus the fp32 accumulation
+//                     of the wgmma chain.  Rows that fail the proof go on a list.
 //   3. k_topk_fallback  persistent, normally finds the list empty: recomputes a listed row's 'd_sae' pre-activations exactly and
 //                     selects from all of them.  Correctness therefore never depends on the approximation; only speed does.
 // Outputs are those of pb_sae_topk: idx int32 / val fp32 [rows][k] sorted by value, feat_count[f] += selections.
@@ -35,8 +38,7 @@ __device__ __forceinline__ bool key_gt_f(float va, int ia, float vb, int ib) { r
 constexpr int FZ_SEG = 128;                       // features per segment: the keys of a segment carry the column in 7 bits
 constexpr int FZ_BM = 128;                        // tile rows: two consumer warpgroups of 64 tokens
 constexpr int FZ_BN = 2 * FZ_SEG;                 // tile columns: two segments, one m64n256 accumulator (128 registers) per thread
-constexpr int FZ_BK = 32;                         // fp32 elements per 128-byte k-slab
-constexpr int FZ_KSTEPS = 4;                      // one wgmma consumes 8 fp32 (32 bytes) of K per row
+constexpr int FZ_KSTEPS = 4;                      // one wgmma consumes 32 bytes of K per row: 8 fp32 (tf32 k8) or 16 fp16 (k16)
 constexpr int FZ_A_BYTES = FZ_BM * 128;           // 16 KB
 constexpr int FZ_STAGE_BYTES = FZ_A_BYTES + FZ_BN * 128;   // + 32 KB of W_encT
 constexpr int FZ_STAGES = 4;                      // 4 x 48 KB = 192 KB operand ring
@@ -74,10 +76,13 @@ __device__ __forceinline__ void key_top8_of32(int (&v)[32]) {
   key_merge8(v, v + 16);
 }
 
-template <int C_KEEP>
+// T = float: tf32 wgmma on the fp32 operands; T = __half: fp16 wgmma on their fp16 copies.  A stage is a 128-byte k-slab of
+// both operands either way (32 fp32 or 64 fp16 elements of K).
+template <int C_KEEP, typename T>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 k_enc_cand(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, int K, int M, int N,
            const float* __restrict__ bias, int* __restrict__ cand, int num_m_tiles, int num_n_tiles) {
+  constexpr int FZ_BK = 128 / sizeof(T);
   pb_pdl_trigger();
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem0 = smem_u32(smem_raw);
@@ -125,7 +130,7 @@ k_enc_cand(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
     }
     return;
   }
-  // ===================== consumers: one tf32 pass, then per-row top-C_KEEP of each segment as packed keys =====================
+  // ===================== consumers: one pass, then per-row top-C_KEEP of each segment as packed keys =====================
   reg_alloc<232>();
   const int c = wg - 1, wq = warp & 3, tid = threadIdx.x & 127;
   float acc[128];
@@ -141,7 +146,10 @@ k_enc_cand(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
       const uint32_t sb = ring + s * FZ_STAGE_BYTES + FZ_A_BYTES;
       wgmma_fence();
 #pragma unroll
-      for (int k = 0; k < FZ_KSTEPS; ++k) wgmma_tf32_n256(acc, make_smem_desc(sa + 32 * k), make_smem_desc(sb + 32 * k), (kb | k) != 0 ? 1u : 0u);
+      for (int k = 0; k < FZ_KSTEPS; ++k) {
+        if constexpr (sizeof(T) == 2) wgmma_f16_n256(acc, make_smem_desc(sa + 32 * k), make_smem_desc(sb + 32 * k), (kb | k) != 0 ? 1u : 0u);
+        else wgmma_tf32_n256(acc, make_smem_desc(sa + 32 * k), make_smem_desc(sb + 32 * k), (kb | k) != 0 ? 1u : 0u);
+      }
       wgmma_commit();
       wgmma_wait<1>();
       if (prev_s >= 0 && tid == 0) mbar_arrive(empty_bar(prev_s));
@@ -244,7 +252,8 @@ __device__ __forceinline__ int sel_pos(unsigned long long it) { return (int)(0xF
 template <int SPT>
 __global__ void __launch_bounds__(256) k_cand_select(const int* __restrict__ cand, int nseg, int c_keep, const float* __restrict__ sae_in,
                                                      const float* __restrict__ W_encT, const float* __restrict__ b_enc,
-                                                     const float* __restrict__ wnorm_max, float err_scale, int d, int k, int m_cand,
+                                                     const float* __restrict__ wnorm_max, const float* __restrict__ wlo_max, int f16,
+                                                     float acc_units, float err_scale, int d, int k, int m_cand,
                                                      int* __restrict__ out_idx, float* __restrict__ out_val, float* __restrict__ feat_count,
                                                      int* __restrict__ fb_count, int* __restrict__ fb_rows, int* __restrict__ stats) {
   pb_pdl();
@@ -261,7 +270,7 @@ __global__ void __launch_bounds__(256) k_cand_select(const int* __restrict__ can
   const int nvec = d >> 2;
   const int nkeys = nseg * c_keep;
 
-  // ---- the token's encoder input -> shared memory; ||a|| and ||a - tf32_trunc(a)|| for the error bound
+  // ---- the token's encoder input -> shared memory; ||a|| and ||a - read(a)|| (tf32 truncation or fp16 rounding) for the error bound
   {
     const float4* src = reinterpret_cast<const float4*>(sae_in + (int64_t)row * d);
     float4* dst = reinterpret_cast<float4*>(a_row);
@@ -270,8 +279,13 @@ __global__ void __launch_bounds__(256) k_cand_select(const int* __restrict__ can
       const float4 v = src[i];
       dst[i] = v;
       nsq += v.x * v.x + v.y * v.y + v.z * v.z + v.w * v.w;
-      const float lx = v.x - tf32_trunc(v.x), ly = v.y - tf32_trunc(v.y), lz = v.z - tf32_trunc(v.z), lw = v.w - tf32_trunc(v.w);
-      lsq += lx * lx + ly * ly + lz * lz + lw * lw;
+      if (f16) {
+        const float q[4] = {v.x, v.y, v.z, v.w};
+        f16x4(q, lsq);
+      } else {
+        const float lx = v.x - tf32_trunc(v.x), ly = v.y - tf32_trunc(v.y), lz = v.z - tf32_trunc(v.z), lw = v.w - tf32_trunc(v.w);
+        lsq += lx * lx + ly * ly + lz * lz + lw * lw;
+      }
     }
     nsq = warp_sum(nsq);
     lsq = warp_sum(lsq);
@@ -421,12 +435,13 @@ __global__ void __launch_bounds__(256) k_cand_select(const int* __restrict__ can
       const int u_rest = m_cur < G ? sel_key(items[m_cur]) : u_below;                      // best key not re-scored
       const int u = max(u_rest, sat_key);
       const float u_val = u == INT_MIN ? -INFINITY : ord2f((u & ~127) | 127);               // upper end of the key's value bucket
-      // |tf32 product - exact| = |a_lo.w + a_hi.w_lo| <= ||a_lo|| max||w|| + ||a|| max||w_lo||   (Cauchy-Schwarz, per row)
-      // + the fp32 accumulation of the wgmma chain: ceil(d / 8) k-steps, each allowed 4 units of 2^-23 of the magnitudes entering it
-      //   (accumulator and eight products: a step that truncates instead of rounding costs 2, the rest is margin), every one of
-      //   them bounded by sum_i |a_i w_i| <= ||a|| max||w||
-      const float acc_err = (float)((d + 7) / 8) * 4.76837158e-7f * a_norm * wnorm_max[0];
-      const float E = err_scale * (a_lo_norm * wnorm_max[0] + a_norm * wnorm_max[1]) + acc_err + fabsf(tau_exact) * 1.2207031e-4f;
+      // |one-pass product - exact| = |a_lo.w + a_hi.w_lo| <= ||a_lo|| max||w|| + ||a|| max||w_lo||   (Cauchy-Schwarz, per row;
+      // a_hi / w_hi = what the tensor core reads, a_lo / w_lo = the residuals)
+      // + the fp32 accumulation of the wgmma chain: acc_units = ceil(d / 8) tf32 k-steps x 4 units of 2^-23, or ceil(d / 16) fp16
+      //   k-steps x 8 units, of the magnitudes entering a step (accumulator and 8 or 16 products: an alignment that truncates
+      //   instead of rounding costs 2 units, the rest is margin), every one of them bounded by sum_i |a_i w_i| <= ||a|| max||w||
+      const float acc_err = acc_units * 1.19209290e-7f * a_norm * wnorm_max[0];
+      const float E = err_scale * (a_lo_norm * wnorm_max[0] + a_norm * wlo_max[0]) + acc_err + fabsf(tau_exact) * 1.2207031e-4f;
       ok = !overflow && m_cur >= k && (u_val + E < tau_exact);
     }
     if (ok || m_cur >= Gs) break;
@@ -540,12 +555,30 @@ __global__ void __launch_bounds__(256) k_rownorm_max(const float* __restrict__ W
   }
 }
 
-template <int C_KEEP>
+// W16 = fp16 copy of W [rows][d]; lo_max[0] = max_r ||W[r,:] - W16[r,:]|| (atomic max on the bit patterns; zeroed by the caller)
+__global__ void __launch_bounds__(256) k_f16_copy(const float* __restrict__ W, int64_t rows, int d, __half* __restrict__ W16, float* __restrict__ lo_max) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+  const int nvec = d >> 2;
+  float best = 0.f;
+  for (int64_t r = (int64_t)blockIdx.x * nw + warp; r < rows; r += (int64_t)gridDim.x * nw) {
+    float l = 0.f;
+    for (int i = lane; i < nvec; i += 32) {
+      float v[4];
+      ld4(W + r * d + 4 * i, v);
+      *reinterpret_cast<uint2*>(W16 + r * d + 4 * i) = f16x4(v, l);
+    }
+    best = fmaxf(best, warp_sum(l));
+  }
+  if (lo_max && lane == 0 && best > 0.f) atomicMax(reinterpret_cast<unsigned int*>(lo_max), __float_as_uint(sqrtf(best)));
+}
+
+template <int C_KEEP, typename T>
 int launch_enc_cand(const PbSaeEncode* e, cudaStream_t st) {
+  constexpr bool F16 = sizeof(T) == 2;
   CUtensorMap tmA, tmB;
-  PB_TRY(make_map(&tmA, e->sae_in, PB_F32, e->rows, e->d, e->d, FZ_BM));
-  PB_TRY(make_map(&tmB, e->W_encT, PB_F32, e->F, e->d, e->d, FZ_BN));
-  auto kern = k_enc_cand<C_KEEP>;
+  PB_TRY(make_map(&tmA, F16 ? e->sae_in16 : (const void*)e->sae_in, F16 ? PB_F16 : PB_F32, e->rows, e->d, e->d, FZ_BM));
+  PB_TRY(make_map(&tmB, F16 ? e->W_encT16 : (const void*)e->W_encT, F16 ? PB_F16 : PB_F32, e->F, e->d, e->d, FZ_BN));
+  auto kern = k_enc_cand<C_KEEP, T>;
   static bool attr_done = false;
   if (!attr_done) {
     PB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, FZ_SMEM));
@@ -559,10 +592,12 @@ int launch_enc_cand(const PbSaeEncode* e, cudaStream_t st) {
 }
 
 template <int SPT>
-int launch_select(const PbSaeEncode* e, int nseg, float scale, cudaStream_t st) {
+int launch_select(const PbSaeEncode* e, bool f16, int nseg, float scale, cudaStream_t st) {
   const size_t smem = sizeof(float) * e->d;
-  PB_LAUNCH_PDL(k_cand_select<SPT>, e->rows, 256, smem, st, (const int*)e->cand, nseg, e->c_keep, e->sae_in, e->W_encT, e->b_enc, e->enc_norm_max, scale,
-                e->d, e->k, e->m_cand, e->idx, e->val, e->feat_count, e->fb_count, e->fb_rows, e->fb_count + 1);
+  const float acc_units = f16 ? 8.f * (float)((e->d + 15) / 16) : 4.f * (float)((e->d + 7) / 8);
+  PB_LAUNCH_PDL(k_cand_select<SPT>, e->rows, 256, smem, st, (const int*)e->cand, nseg, e->c_keep, e->sae_in, e->W_encT, e->b_enc, e->enc_norm_max,
+                f16 ? e->enc16_lo_max : e->enc_norm_max + 1, (int)f16, acc_units, scale, e->d, e->k, e->m_cand, e->idx, e->val, e->feat_count,
+                e->fb_count, e->fb_rows, e->fb_count + 1);
   return PB_OK;
 }
 
@@ -589,21 +624,32 @@ extern "C" int pb_sae_encode_topk_fused(const PbSaeEncode* e, pb_stream_t stream
   const int nkeys = e->F / FZ_SEG * e->c_keep;
   PB_CHECK_ARG(e->F / FZ_SEG <= 256 * 4, "pb_sae_encode_topk_fused: d_sae=%d too large for the selection kernel (max 131072)", e->F);
   PB_CHECK_ARG(e->cand_bytes >= (int64_t)e->rows * nkeys * 4, "pb_sae_encode_topk_fused: candidate buffer too small");
+  const bool f16 = e->sae_in16 != nullptr;
+  PB_CHECK_ARG(f16 == (e->W_encT16 != nullptr) && f16 == (e->enc16_lo_max != nullptr),
+               "pb_sae_encode_topk_fused: sae_in16, W_encT16 and enc16_lo_max go together");
+  PB_CHECK_ARG(!f16 || (e->d % 8 == 0 && pb_aligned16(e->sae_in16) && pb_aligned16(e->W_encT16)),
+               "pb_sae_encode_topk_fused: the fp16 candidate GEMM needs d_in %% 8 == 0 and 16-byte aligned fp16 operands (d=%d)", e->d);
   if (e->rows == 0) return PB_OK;
   cudaStream_t st = (cudaStream_t)stream;
   const int phases = (e->phases & 7) ? e->phases : (e->phases | 7);
   if (phases & 1) {
-    if (e->c_keep == 4) PB_TRY(launch_enc_cand<4>(e, st));
-    else if (e->c_keep == 6) PB_TRY(launch_enc_cand<6>(e, st));
-    else PB_TRY(launch_enc_cand<8>(e, st));
+    if (f16) {
+      if (e->c_keep == 4) PB_TRY((launch_enc_cand<4, __half>(e, st)));
+      else if (e->c_keep == 6) PB_TRY((launch_enc_cand<6, __half>(e, st)));
+      else PB_TRY((launch_enc_cand<8, __half>(e, st)));
+    } else {
+      if (e->c_keep == 4) PB_TRY((launch_enc_cand<4, float>(e, st)));
+      else if (e->c_keep == 6) PB_TRY((launch_enc_cand<6, float>(e, st)));
+      else PB_TRY((launch_enc_cand<8, float>(e, st)));
+    }
   }
   if (phases & 2) {
     if (!(phases & 8)) PB_CUDA(cudaMemsetAsync(e->fb_count, 0, 2 * sizeof(int), st));    // [0] rows on the exact path, [1] candidates re-scored
     const float coef = e->err_coef > 0.f ? e->err_coef : 1.05f;       // safety factor on the Cauchy-Schwarz bound (norms evaluated in fp32)
     const int nseg = e->F / FZ_SEG, spt = (nseg + 255) / 256;
-    if (spt <= 1) PB_TRY(launch_select<1>(e, nseg, coef, st));
-    else if (spt <= 2) PB_TRY(launch_select<2>(e, nseg, coef, st));
-    else PB_TRY(launch_select<4>(e, nseg, coef, st));
+    if (spt <= 1) PB_TRY(launch_select<1>(e, f16, nseg, coef, st));
+    else if (spt <= 2) PB_TRY(launch_select<2>(e, f16, nseg, coef, st));
+    else PB_TRY(launch_select<4>(e, f16, nseg, coef, st));
   }
   if (phases & 4) {
     PB_CHECK_ARG(e->fb_scratch && e->fb_scratch_bytes >= (int64_t)e->F * 4, "pb_sae_encode_topk_fused: fallback scratch missing");
@@ -632,6 +678,18 @@ extern "C" int pb_rownorm_max(const float* W, int32_t F, int32_t d, float* out, 
   int grid = pb_sm_count() * 4;
   if (grid > (F + 7) / 8) grid = (F + 7) / 8;
   k_rownorm_max<<<grid, 256, 0, st>>>(W, F, d, out);
+  PB_LAUNCH_CHECK();
+  return PB_OK;
+}
+
+extern "C" int pb_f16_copy(const float* W, int64_t rows, int32_t d, void* W16, float* lo_max, pb_stream_t stream) {
+  PB_CHECK_ARG(W && W16 && rows >= 0 && d > 0 && d % 4 == 0 && pb_aligned16(W) && ((uintptr_t)W16 & 7) == 0, "pb_f16_copy: bad arguments");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (lo_max) PB_CUDA(cudaMemsetAsync(lo_max, 0, sizeof(float), st));
+  if (rows == 0) return PB_OK;
+  int64_t grid = (rows + 7) / 8;
+  if (grid > pb_sm_count() * 4) grid = pb_sm_count() * 4;
+  k_f16_copy<<<(int)grid, 256, 0, st>>>(W, rows, d, (__half*)W16, lo_max);
   PB_LAUNCH_CHECK();
   return PB_OK;
 }

@@ -74,12 +74,13 @@ __device__ __forceinline__ void dead_feature_counters(float* since_fired, float*
 // ---------------------------------------------------------------------------------------------
 // The update of one feature by one warp (lane l holds columns 4 (i * 32 + l) .. +3 of chunk i).  The row pointers (parameters,
 // gradients, Adam moments; global or shared memory) are read; the moments are written back in place; the updated parameter rows
-// go to out.dec(c4, w) / out.enc(c4, p, lo) (lo = tf32 residual of p), which decide where they are stored.  Returns this lane's
-// partials of ||w_enc||^2 and ||w_enc - trunc(w_enc)||^2 (the fused encoder's error bound) in esq / elo.
+// go to out.dec(c4, w) / out.enc(c4, p, lo, p16) (lo = tf32 residual of p, p16 = fp16 copy of p, packed), which decide where they
+// are stored.  Returns this lane's partials of ||w_enc||^2, ||w_enc - trunc(w_enc)||^2 and ||w_enc - fp16(w_enc)||^2 (the fused
+// encoder's error bounds) in esq / elo / e16; a caller that stores no fp16 copy ignores e16 and the compiler drops its arithmetic.
 template <int CHUNKS, class Out>
 __device__ __forceinline__ void sae_adam_feature(const float* wd, const float* gd, float* md, float* vd, const float* we, const float* ge,
                                                  float* me, float* ve, float clip, const AdamHyper& h, int nvec, bool renorm,
-                                                 const Out& out, float& esq, float& elo) {
+                                                 const Out& out, float& esq, float& elo, float& e16) {
   const int lane = threadIdx.x & 31;
   // ---- decoder row: clip, remove the component parallel to the (unit-norm) row, Adam, renormalise
   float w[CHUNKS][4], gq[CHUNKS][4];
@@ -129,6 +130,7 @@ __device__ __forceinline__ void sae_adam_feature(const float* wd, const float* g
   // ---- encoder row (feature-major)
   esq = 0.f;
   elo = 0.f;
+  e16 = 0.f;
 #pragma unroll
   for (int i = 0; i < CHUNKS; ++i) {
     const int c4 = i * 32 + lane;
@@ -148,7 +150,7 @@ __device__ __forceinline__ void sae_adam_feature(const float* wd, const float* g
       }
       st4(me + 4 * c4, mm);
       st4(ve + 4 * c4, vv);
-      out.enc(c4, p, lo);
+      out.enc(c4, p, lo, f16x4(p, e16));
     }
   }
 }

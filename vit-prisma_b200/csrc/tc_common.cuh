@@ -84,6 +84,16 @@ __device__ __forceinline__ void wgmma_tf32_n256(float (&d)[128], uint64_t adesc,
       : PB_ACC128_OUT
       : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
+// D[64 x 256] (+)= A[64 x 16] * B[256 x 16]^T, fp16 operands, fp32 accumulation
+__device__ __forceinline__ void wgmma_f16_n256(float (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 "
+      "{" PB_ACC128_REGS "}, "
+      "%128, %129, p, 1, 1, 0, 0;\n\t}"
+      : PB_ACC128_OUT
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
 __device__ __forceinline__ void wgmma_bf16_n128(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
@@ -153,12 +163,14 @@ EncodeTiledFn get_encode_fn() {
 int make_map(CUtensorMap* map, const void* ptr, int dtype, int64_t rows, int64_t cols, int64_t ld, int box_rows) {
   EncodeTiledFn fn = get_encode_fn();
   if (!fn) { pb_set_error("gemm_tc: cuTensorMapEncodeTiled entry point unavailable"); return PB_ECUDA; }
-  const int es = dtype == PB_BF16 ? 2 : 4;
+  const int es = dtype == PB_F32 ? 4 : 2;
   cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
   cuuint64_t gstride[1] = {(cuuint64_t)ld * es};
   cuuint32_t box[2] = {(cuuint32_t)(128 / es), (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult rc = fn(map, dtype == PB_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(ptr), gdim,
+  const CUtensorMapDataType dt = dtype == PB_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                 : dtype == PB_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+  CUresult rc = fn(map, dt, 2, const_cast<void*>(ptr), gdim,
                    gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (rc != CUDA_SUCCESS) {

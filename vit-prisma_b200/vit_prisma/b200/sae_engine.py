@@ -40,6 +40,7 @@ class PbSaeStep(C.Structure):
             "fired", "scalars", "m_dec", "v_dec", "m_enc", "v_enc", "m_be", "v_be", "m_bd", "v_bd",
             "since_fired", "act_freq")]
         + [("global_rows", i32), ("dist", i32), ("work", vp), ("work_bytes", i64), ("enc_norm_max", vp), ("pre_zeroed", i32)]
+        + [("W_encT16", vp), ("enc16_lo_max", vp)]
     )
 
 
@@ -49,12 +50,15 @@ class PbSaeEncode(C.Structure):
         [(n, i32) for n in ("rows", "d", "F", "k", "c_keep", "m_cand", "phases")] + [("err_coef", f32)]
         + [(n, vp) for n in ("sae_in", "W_encT", "b_enc", "enc_norm_max", "cand")] + [("cand_bytes", i64)]
         + [(n, vp) for n in ("idx", "val", "feat_count", "fb_count", "fb_rows", "fb_scratch")] + [("fb_scratch_bytes", i64)]
+        + [(n, vp) for n in ("sae_in16", "W_encT16", "enc16_lo_max")]
     )
 
 
 L.ABI_STRUCTS.append(PbSaeStep)
 L.register_signatures({
     "pb_sae_prep": (i32, [vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, vp]),
+    "pb_sae_prep16": (i32, [vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, vp]),
+    "pb_f16_copy": (i32, [vp, i64, i32, vp, vp, vp]),
     "pb_sae_topk": (i32, [vp, i32, i32, i32, vp, vp, vp, vp, i64, vp]),
     "pb_sae_scatter_acts": (i32, [vp, vp, vp, i32, i32, i32, i32, vp]),
     "pb_sae_step_reset": (i32, [C.POINTER(PbSaeStep), vp, vp]),
@@ -156,17 +160,28 @@ class SaeStepEngine:
         # encoder route: "fused" = one-pass tf32 GEMM with a candidate epilogue + exact re-scoring (csrc/sae_fused.cu, no dense
         # hidden_pre); "dense" = fp32-grade GEMM -> hidden_pre -> k_topk.  "auto" picks fused whenever the geometry allows it and
         # the caller did not pin a GEMM implementation.
+        # Candidate-GEMM operands of the fused route (cand_operands): "f16" = fp16 copies of sae_in / W_enc (the 11-bit significand
+        # of tf32 at half the bytes of the L2-bound operand stream), taken by "auto" on one GPU when d_in % 8 == 0 and d_in >= 64;
+        # "tf32" = the fp32 operands read as tf32, for an explicit encoder="fused" and the data-parallel engine (whose all-gather
+        # carries no fp16 copy).
         fused_ok = self.d % 4 == 0 and self.d >= 32 and self.F % 128 == 0 and self.k <= 48 and self.F <= 131072
+        f16_ok = encoder == "auto" and self.d % 8 == 0 and self.d >= 64 and not self.is_data_parallel
         if encoder == "auto":
             encoder = "fused" if (fused_ok and gemm_impl == L.GEMM_AUTO) else "dense"
         if encoder == "fused" and not fused_ok:
             raise L.PrismaB200Error(f"fused encoder->TopK needs d_in % 4 == 0, d_sae % 128 == 0, k <= 48 (d={self.d} F={self.F} k={self.k})")
+        self.cand_operands = ("f16" if f16_ok else "tf32") if encoder == "fused" else None
         import os
         self.encoder, self.c_keep = encoder, int(os.environ.get("PRISMA_SAE_C_KEEP", c_keep))     # env overrides: tuning runs only
         self.m_cand = int(os.environ.get("PRISMA_SAE_M_CAND", 0)) or (int(m_cand) if m_cand else self.k + 8)   # first round; +16 per round while unproven
         self.enc_norm_max = z(2)                      # max ||w_f||, max ||w_f - tf32_trunc(w_f)|| (error bound of the fused encoder)
         self.fb_count = z(2, dt=torch.int32)          # rows on the exact path, candidates re-scored (last fused encode)
         self.W_encT_lo = torch.empty_like(W_encT) if encoder == "dense" else None
+        # fp16 route: the fp16 copy of W_enc the candidate GEMM reads, and max ||w_f - fp16(w_f)|| for its error bound; pb_sae_adam
+        # rewrites both with every update, refresh_lo() after any other write to W_enc
+        f16 = self.cand_operands == "f16"
+        self.W_encT16 = torch.empty(self.F, self.d, dtype=torch.float16, device=dev) if f16 else None
+        self.enc16_lo_max = z(1) if f16 else None
         self.refresh_lo()
         # optimizer state (torch.optim.Adam: exp_avg / exp_avg_sq start at zero)
         self.m_dec, self.v_dec, self.m_enc, self.v_enc = z(self.F, self.d), z(self.F, self.d), z(self.F, self.d), z(self.F, self.d)
@@ -183,11 +198,15 @@ class SaeStepEngine:
 
     def refresh_lo(self) -> None:
         """Recompute what the encoder kernels derive from W_enc (after an external write to the parameters): the tf32 residual
-        plane of the dense 3xTF32 route, the largest encoder-column norm of the fused route's error bound."""
+        plane of the dense 3xTF32 route, the largest encoder-column norms of the fused route's error bound, and the fp16 copy
+        of W_enc (+ its residual norm) on the fp16 candidate route.  A stale copy would make the bound describe another matrix."""
         if self.W_encT_lo is not None:
             from . import ops
             self.W_encT_lo.copy_(ops.split_tf32(self.W_encT))
         L.check(L.get_lib().pb_rownorm_max(self.W_encT.data_ptr(), self.F, self.d, self.enc_norm_max.data_ptr(), _stream()), "pb_rownorm_max")
+        if self.W_encT16 is not None:
+            L.check(L.get_lib().pb_f16_copy(self.W_encT.data_ptr(), self.F, self.d, self.W_encT16.data_ptr(), self.enc16_lo_max.data_ptr(),
+                                            _stream()), "pb_f16_copy")
 
     def _ensure_rows(self, rows: int) -> None:
         if rows == self._rows:
@@ -203,6 +222,7 @@ class SaeStepEngine:
             self.fb_rows = e(max(rows, 1), dt=torch.int32)
             self.fb_scratch = e(min(64, max(sb.value // (4 * F), 1)) * F)      # exact path: one d_sae row per resident CTA
             self.sae_in_lo = self.hidden_pre = None
+            self.sae_in16 = e(rows, d, dt=torch.float16) if self.cand_operands == "f16" else None
         else:
             self.sae_in_lo, self.hidden_pre = e(rows, d), e(rows, F)
         self.idx, self.val, self.dval = e(rows, k, dt=torch.int32), e(rows, k), e(rows, k)
@@ -231,6 +251,7 @@ class SaeStepEngine:
         s.since_fired, s.act_freq = p(since_fired), p(act_freq)
         s.work, s.work_bytes = p(self.work), self.work.numel()
         s.enc_norm_max = p(self.enc_norm_max)
+        s.W_encT16, s.enc16_lo_max = p(self.W_encT16), p(self.enc16_lo_max)
         return s
 
     def _enc_desc(self, rows: int, phases: int = 0) -> PbSaeEncode:
@@ -241,6 +262,8 @@ class SaeStepEngine:
         e.idx, e.val, e.feat_count = self.idx.data_ptr(), self.val.data_ptr(), self.feat_count.data_ptr()
         e.fb_count, e.fb_rows = self.fb_count.data_ptr(), self.fb_rows.data_ptr()
         e.fb_scratch, e.fb_scratch_bytes = self.fb_scratch.data_ptr(), self.fb_scratch.numel() * 4
+        if self.cand_operands == "f16":
+            e.sae_in16, e.W_encT16, e.enc16_lo_max = self.sae_in16.data_ptr(), self.W_encT16.data_ptr(), self.enc16_lo_max.data_ptr()
         return e
 
     # ------------------------------------------------------------------ pieces
@@ -262,10 +285,14 @@ class SaeStepEngine:
         lib, st = L.get_lib(), _stream()
         rows = x.shape[0]
         self._ensure_rows(rows)
-        L.check(lib.pb_sae_prep(x.data_ptr(), self.b_dec.data_ptr(), self.sae_in.data_ptr(),
-                                self.sae_in_lo.data_ptr() if (self.sae_in_lo is not None and self.gemm_impl != L.GEMM_SIMT) else None,
-                                self.mu.data_ptr(), self.sd.data_ptr(),
-                                self.xsum.data_ptr(), rows, self.d, self.norm_mode, st), "pb_sae_prep")
+        if self.cand_operands == "f16":                # + the fp16 copy of sae_in the candidate GEMM reads
+            L.check(lib.pb_sae_prep16(x.data_ptr(), self.b_dec.data_ptr(), self.sae_in.data_ptr(), self.sae_in16.data_ptr(), self.mu.data_ptr(),
+                                      self.sd.data_ptr(), self.xsum.data_ptr(), rows, self.d, self.norm_mode, st), "pb_sae_prep16")
+        else:
+            L.check(lib.pb_sae_prep(x.data_ptr(), self.b_dec.data_ptr(), self.sae_in.data_ptr(),
+                                    self.sae_in_lo.data_ptr() if (self.sae_in_lo is not None and self.gemm_impl != L.GEMM_SIMT) else None,
+                                    self.mu.data_ptr(), self.sd.data_ptr(),
+                                    self.xsum.data_ptr(), rows, self.d, self.norm_mode, st), "pb_sae_prep")
         if not pre_zeroed:
             self.feat_count.zero_()
         if self.encoder == "fused":
@@ -309,7 +336,8 @@ class SaeStepEngine:
     # ------------------------------------------------------------------ instrumentation (bench.py / tools)
     def describe_encoder(self) -> str:
         if self.encoder == "fused":
-            return (f"fused: one-pass tf32 wgmma GEMM with top-{self.c_keep}-per-128-features epilogue -> exact fp32 re-scoring of "
+            ops_ = "fp16 copies of the operands" if self.cand_operands == "f16" else "tf32"
+            return (f"fused: one-pass wgmma GEMM ({ops_}) with top-{self.c_keep}-per-128-features epilogue -> exact fp32 re-scoring of "
                     f">= {self.m_cand} candidates per token -> exact top-{self.k} with a completeness proof (no dense hidden_pre)")
         return "wgmma 3xTF32 GEMM -> dense hidden_pre -> exact k_topk" if self.gemm_impl != L.GEMM_SIMT else "exact FFMA GEMM -> k_topk"
 
@@ -326,8 +354,9 @@ class SaeStepEngine:
         """(name, callable, info) of the stages after backward; the data-parallel engine replaces them with its peer-memory phases."""
         lib, st = L.get_lib(), _stream()
         kernel = "k_sae_adam_rows" if self.W_encT_lo is not None or self.d < 64 else "k_sae_adam_bulk"   # pb_sae_adam's choice
+        f16_copy = 2 * self.d * self.F if self.W_encT16 is not None else 0      # + the fp16 copy of W_enc
         return [("adam (clip + decoder-parallel-gradient removal + Adam + row renorm)", lambda: L.check(lib.pb_sae_adam(C.byref(s), st)),
-                 dict(bytes=60 * self.d * self.F, ncu=kernel))]
+                 dict(bytes=60 * self.d * self.F + f16_copy, ncu=kernel))]
 
     def _clip_and_adam(self, x: torch.Tensor, lr: float, since_fired, act_freq, grads, extra) -> None:
         """Optimizer tail of the engines whose gradients come from dense products: global norm over ``grads`` -> clip coefficient,
@@ -389,11 +418,12 @@ class SaeStepEngine:
             self.encode_topk(x)
             flops = 2.0 * rows * self.d * self.F
             nkeys = (self.F // 128) * self.c_keep
-            return [("encode + topk, fused (prep + tf32 candidate GEMM + select / exact re-score + exact path)", lambda: self.encode_topk(x),
+            op, es = ("fp16", 2) if self.cand_operands == "f16" else ("tf32", 4)
+            return [(f"encode + topk, fused (prep + {op} candidate GEMM + select / exact re-score + exact path)", lambda: self.encode_topk(x),
                      dict(flops=flops, passes=1)),
-                    ("candidate GEMM alone (one tf32 pass, top-c-per-segment epilogue)",
+                    (f"candidate GEMM alone (one {op} pass, top-c-per-segment epilogue)",
                      lambda: L.check(lib.pb_sae_encode_topk_fused(C.byref(self._enc_desc(rows, 1)), st)),
-                     dict(flops=flops, passes=1, bytes=4 * self.d * self.F + 4 * rows * self.d + 4 * rows * nkeys, ncu=r"k_enc_cand")),
+                     dict(flops=flops, passes=1, bytes=es * self.d * self.F + es * rows * self.d + 4 * rows * nkeys, ncu=r"k_enc_cand")),
                     ("select + exact re-score alone", lambda: L.check(lib.pb_sae_encode_topk_fused(C.byref(self._enc_desc(rows, 2)), st)),
                      dict(bytes=4 * rows * nkeys + 4 * rows * self.d + 8 * rows * self.k, ncu=r"k_cand_select"))]
         return [("encode + topk (prep + encoder GEMM 3xTF32 + exact topk)", lambda: self.encode_topk(x),
