@@ -134,6 +134,10 @@ PB_API int pb_mean_tokens(const void* x, void* out, int32_t B, int32_t T, int32_
 /* images [B,C,S,S] -> patches [B*(S/P)^2, C*P*P] in conv-weight order (patch_embedding.py:26-32) */
 PB_API int pb_im2col_patches(const void* images, void* patches, int32_t B, int32_t C, int32_t S,
                       int32_t P, int32_t dtype, pb_stream_t s);
+/* video [B,C,F,S,S] -> patches [B*(F/D)*(S/P)^2, C*D*P*P] in Conv3d-weight order, tokens (t, h, w) with t slowest;
+ * frames past (F/D)*D are dropped as Conv3d drops them (patch_embedding.py:36-62).  D = F = 1 is pb_im2col_patches. */
+PB_API int pb_im2col_tubelets(const void* images, void* patches, int32_t B, int32_t C, int32_t F, int32_t S,
+                       int32_t P, int32_t D, int32_t dtype, pb_stream_t s);
 /* full[b,0,:] = cls + pos[0];  full[b,1+i,:] = embed[b,i,:] + pos[1+i]  (base_vit.py:171-179)
  * with use_cls == 0: full[b,i,:] = embed[b,i,:] + pos[i]                                  */
 PB_API int pb_embed_assemble(const void* embed, const void* cls, const void* pos, void* full,
@@ -182,7 +186,7 @@ typedef struct {
   const void *lnpre_w, *lnpre_b, *lnf_w, *lnf_b, *head_w, *head_w_lo, *head_b;
   const PbVitLayerW* layers_host;        /* HOST array [n_layers_run] */
   /* spill destinations / work buffers */
-  void* patches;             /* [B*n_patches, C*P*P] im2col scratch                         */
+  void* patches;             /* [B*n_patches, C*D*P*P] im2col scratch (D = tubelet_depth, 1 for images) */
   void* embed;               /* hook_embed [B,n_patches,d]                                  */
   void* full_embed;          /* hook_full_embed == residual before ln_pre [B,T,d]           */
   float* lnpre_scale; float* lnpre_norm_f32; void* lnpre_out;    /* residual fed to block 0 */
@@ -191,8 +195,11 @@ typedef struct {
   void* pooled;              /* [B,d] cls/gaap-pooled ln_final output                       */
   void* pre_normalize;       /* hook_post_head_pre_normalize [B, n_classes or d]            */
   void* out;                 /* model output                                                */
-  float* lo_scratch;         /* fp32 [max(B*T*(d + max(d_mlp, H*dh)), B*n_patches*C*P*P)]: tf32 residuals of the
+  float* lo_scratch;         /* fp32 [max(B*T*(d + max(d_mlp, H*dh)), B*n_patches*C*D*P*P)]: tf32 residuals of the
                                 GEMM A operands in 3xTF32 mode, or NULL (then fp32 GEMMs run on the exact FFMA path) */
+  /* video towers: images is [B,C,n_frames,S,S] and n_patches = (S/P)^2 * (n_frames / tubelet_depth);
+   * tubelet_depth == 0 means an image model ([B,C,S,S], n_frames unused)                    */
+  int32_t n_frames, tubelet_depth;
 } PbVitForward;
 PB_API int pb_vit_forward(const PbVitForward* f, pb_stream_t stream);
 

@@ -19,6 +19,8 @@
 #include <stdlib.h>
 
 int pb_attention_mma(const PbAttention* p, cudaStream_t st);  // attention_mma.cu
+int pb_attn_scores_long(const PbAttention* p, cudaStream_t st);  // attention_long.cu
+int pb_attn_pv_long(const PbAttention* p, cudaStream_t st);
 
 enum { ATT_FUSED = 0, ATT_SCORES = 1, ATT_PV = 2 };
 
@@ -225,6 +227,19 @@ static int check_att(const PbAttention* p, const char* who) {
   return PB_OK;
 }
 
+// Beyond the 608 tokens of the FFMA kernel the split stages run the tensor-core modes of attention_long.cu, which exist for
+// d_head == 64 only.  Up to 608 tokens the FFMA kernel keeps serving them, so shorter sequences keep their results.
+constexpr int ATT_SIMT_MAX_T = 608;
+static int split_long(int (*fn)(const PbAttention*, cudaStream_t), const PbAttention* p, cudaStream_t st, const char* who) {
+  if (p->dh != 64) {
+    pb_set_error("%s: T=%d with d_head=%d unsupported: beyond %d tokens only d_head 64 is supported", who, p->T, p->dh, ATT_SIMT_MAX_T);
+    return PB_EUNSUPPORTED;
+  }
+  const int rc = fn(p, st);
+  if (rc == PB_EUNSUPPORTED) pb_set_error("%s: T=%d d_head=%d needs 16-byte aligned q/k/v/z pointers", who, p->T, p->dh);
+  return rc;
+}
+
 extern "C" int pb_attention(const PbAttention* p, pb_stream_t stream) {
   PB_TRY(check_att(p, "pb_attention"));
   PB_CHECK_ARG(p->q && p->k && p->v && p->z, "pb_attention: q, k, v, z are required");
@@ -244,12 +259,14 @@ extern "C" int pb_attn_scores(const PbAttention* p, pb_stream_t stream) {
   PB_TRY(check_att(p, "pb_attn_scores"));
   PB_CHECK_ARG(p->q && p->k && p->scores, "pb_attn_scores: q, k, scores are required");
   if (p->B == 0) return PB_OK;
+  if (p->T > ATT_SIMT_MAX_T) return split_long(pb_attn_scores_long, p, (cudaStream_t)stream, "pb_attn_scores");
   return p->dtype == PB_F32 ? launch_att<float, ATT_SCORES>(p, (cudaStream_t)stream) : launch_att<bf16, ATT_SCORES>(p, (cudaStream_t)stream);
 }
 extern "C" int pb_attn_pv(const PbAttention* p, pb_stream_t stream) {
   PB_TRY(check_att(p, "pb_attn_pv"));
   PB_CHECK_ARG(p->pattern && p->v && p->z, "pb_attn_pv: pattern, v, z are required");
   if (p->B == 0) return PB_OK;
+  if (p->T > ATT_SIMT_MAX_T) return split_long(pb_attn_pv_long, p, (cudaStream_t)stream, "pb_attn_pv");
   return p->dtype == PB_F32 ? launch_att<float, ATT_PV>(p, (cudaStream_t)stream) : launch_att<bf16, ATT_PV>(p, (cudaStream_t)stream);
 }
 

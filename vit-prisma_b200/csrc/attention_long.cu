@@ -9,6 +9,12 @@
 // QK^T is computed twice (7.7 MFLOP per image and layer more) in exchange for 32 accumulator registers, 3-6 CTAs per SM and
 // K / V traffic that no longer scales with the number of query slabs per head beyond L2.  Rounding points are the reference's:
 // scores = round(round(q.k) / scale), pattern = round(softmax), z = round(pattern @ v) with the rounded pattern as operand.
+//
+// Two more modes serve the split hooked stages (pb_attn_scores / pb_attn_pv) beyond the 608 tokens of the FFMA kernel:
+//   LONG_SCORES: pass 1 alone, without the softmax statistics -> scores;
+//   LONG_PV:     pass 2 with P read from a [B,H,T,T] pattern in 64-key chunks instead of computed -> z.
+// Both share the fused mode's arithmetic and rounding points, so the scores equal the fused kernel's scores spill bit for bit, and
+// the z of LONG_PV fed the fused kernel's own spilled pattern equals the fused kernel's z bit for bit.
 #include "common.cuh"
 
 namespace {
@@ -53,6 +59,7 @@ __device__ __forceinline__ void ldmatrix_x4_trans(uint32_t (&r)[4], const void* 
 
 constexpr int DH = 64;
 constexpr int KC = 64;                                    // keys per chunk
+enum { LONG_FUSED = 0, LONG_SCORES = 1, LONG_PV = 2 };
 template <typename T> struct Lay { static constexpr int LD = DH + (sizeof(T) == 2 ? 8 : 4); };
 
 __device__ __forceinline__ void stage_put(float* p, float a, float b) { p[0] = a; p[1] = b; }
@@ -73,7 +80,22 @@ __device__ __forceinline__ void copy_rows_out(T* __restrict__ gbase, int64_t row
   }
 }
 
-template <typename T, int NW>
+// nvalid global rows of ncols columns (row stride Tn elements) -> one warp's [16][KC] stage; the rest of the stage is left as is
+template <typename T>
+__device__ __forceinline__ void copy_rows_in(T* stage, const T* __restrict__ gbase, int64_t row_stride, int nvalid, int ncols, int lane) {
+  for (int r = 0; r < nvalid; ++r) {
+    const T* g = gbase + (int64_t)r * row_stride;
+    T* s = stage + r * KC;
+    if (sizeof(T) == 4 || ((reinterpret_cast<uintptr_t>(g) & 3) == 0 && (ncols & 1) == 0)) {
+      const int nw = ncols * (int)sizeof(T) / 4;
+      for (int i = lane; i < nw; i += 32) reinterpret_cast<uint32_t*>(s)[i] = reinterpret_cast<const uint32_t*>(g)[i];
+    } else {
+      for (int i = lane; i < ncols; i += 32) s[i] = g[i];
+    }
+  }
+}
+
+template <typename T, int NW, int MODE>
 __global__ void __launch_bounds__(NW * 32) k_attention_long(const T* __restrict__ q, const T* __restrict__ k, const T* __restrict__ v,
                                                            T* __restrict__ scores, T* __restrict__ pattern, T* __restrict__ z, int Tn, int H,
                                                            float attn_scale, float inv_scale) {
@@ -96,13 +118,15 @@ __global__ void __launch_bounds__(NW * 32) k_attention_long(const T* __restrict_
   const int64_t head_base = (int64_t)b * Tn * tok_stride + (int64_t)h * DH;
   const uint4 zero4 = make_uint4(0u, 0u, 0u, 0u);
 
-  for (int idx = threadIdx.x; idx < NW * 16 * VPR; idx += NW * 32) {
-    const int r = idx / VPR, e = (idx % VPR) * VEC;
-    uint4 qv = zero4;
-    if (row0 + r < Tn) qv = *reinterpret_cast<const uint4*>(q + head_base + (int64_t)(row0 + r) * tok_stride + e);
-    *reinterpret_cast<uint4*>(Qs + (size_t)r * LD + e) = qv;
+  if (MODE != LONG_PV) {
+    for (int idx = threadIdx.x; idx < NW * 16 * VPR; idx += NW * 32) {
+      const int r = idx / VPR, e = (idx % VPR) * VEC;
+      uint4 qv = zero4;
+      if (row0 + r < Tn) qv = *reinterpret_cast<const uint4*>(q + head_base + (int64_t)(row0 + r) * tok_stride + e);
+      *reinterpret_cast<uint4*>(Qs + (size_t)r * LD + e) = qv;
+    }
+    __syncthreads();
   }
-  __syncthreads();
 
   const int wrow0 = row0 + warp * 16;
   const bool active = wrow0 < Tn;                          // inactive warps still load chunks and hit the barriers
@@ -113,7 +137,8 @@ __global__ void __launch_bounds__(NW * 32) k_attention_long(const T* __restrict_
   // ---- Q fragments of this warp, kept in registers for both passes
   uint32_t qa[BF ? DH / 16 : DH / 8][4];                   // bf16: packed pairs; fp32: tf32 hi words
   uint32_t qal[BF ? 1 : DH / 8][4];                        // fp32: tf32 lo words
-  if constexpr (BF) {
+  if constexpr (MODE == LONG_PV) {
+  } else if constexpr (BF) {
 #pragma unroll
     for (int kk = 0; kk < DH / 16; ++kk) ldmatrix_x4(qa[kk], Qw + (size_t)(lane & 15) * LD + kk * 16 + 8 * (lane >> 4));
   } else {
@@ -134,8 +159,10 @@ __global__ void __launch_bounds__(NW * 32) k_attention_long(const T* __restrict_
 #pragma unroll
   for (int nn = 0; nn < DH / 8; ++nn) o[nn][0] = o[nn][1] = o[nn][2] = o[nn][3] = 0.f;
 
+  // LONG_FUSED: passes 0 and 1; LONG_SCORES: pass 0 alone; LONG_PV: pass 1 alone
+  constexpr int PASS_BEGIN = MODE == LONG_PV ? 1 : 0, PASS_END = MODE == LONG_SCORES ? 1 : 2;
 #pragma unroll 1
-  for (int pass = 0; pass < 2; ++pass) {
+  for (int pass = PASS_BEGIN; pass < PASS_END; ++pass) {
 #pragma unroll 1
     for (int c = 0; c < nchunks; ++c) {
       const int kc0 = c * KC;
@@ -144,20 +171,32 @@ __global__ void __launch_bounds__(NW * 32) k_attention_long(const T* __restrict_
         const int j = idx / VPR, e = (idx % VPR) * VEC;
         uint4 kv = zero4, vv = zero4;
         if (kc0 + j < Tn) {
-          kv = *reinterpret_cast<const uint4*>(k + head_base + (int64_t)(kc0 + j) * tok_stride + e);
+          if (MODE != LONG_PV) kv = *reinterpret_cast<const uint4*>(k + head_base + (int64_t)(kc0 + j) * tok_stride + e);
           if (pass == 1) vv = *reinterpret_cast<const uint4*>(v + head_base + (int64_t)(kc0 + j) * tok_stride + e);
         }
-        *reinterpret_cast<uint4*>(Ks + (size_t)j * LD + e) = kv;
+        if (MODE != LONG_PV) *reinterpret_cast<uint4*>(Ks + (size_t)j * LD + e) = kv;
         if (pass == 1) *reinterpret_cast<uint4*>(Vs + (size_t)j * LD + e) = vv;
       }
       __syncthreads();
       if (!active) continue;
 
-      // ---- S chunk = Q K_chunk^T (identical arithmetic in both passes)
+      // ---- S chunk = Q K_chunk^T (identical arithmetic in both passes); LONG_PV: the P chunk from the pattern instead
       float acc[NTC][4];
 #pragma unroll
       for (int nt = 0; nt < NTC; ++nt) acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0.f;
-      if constexpr (BF) {
+      if constexpr (MODE == LONG_PV) {
+        const int pcols = min(KC, Tn - kc0);
+        copy_rows_in<T>(stage, pattern + sc_row0 * Tn + kc0, Tn, nvalid, pcols, lane);
+        __syncwarp();
+#pragma unroll
+        for (int nt = 0; nt < NTC; ++nt)
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const int row = g + (i < 2 ? 0 : 8), col = nt * 8 + 2 * t + (i & 1);
+            acc[nt][i] = (row < nvalid && col < pcols) ? ld_as_float(stage + row * KC + col) : 0.f;
+          }
+        __syncwarp();
+      } else if constexpr (BF) {
 #pragma unroll
         for (int nt = 0; nt < NTC; ++nt) {
 #pragma unroll
@@ -179,7 +218,8 @@ __global__ void __launch_bounds__(NW * 32) k_attention_long(const T* __restrict_
           }
         }
       }
-      if (inv_scale != 0.f) {
+      if (MODE == LONG_PV) {
+      } else if (inv_scale != 0.f) {
 #pragma unroll
         for (int nt = 0; nt < NTC; ++nt)
 #pragma unroll
@@ -193,35 +233,37 @@ __global__ void __launch_bounds__(NW * 32) k_attention_long(const T* __restrict_
       const int ncols = min(KC, Tn - kc0);
 
       if (pass == 0) {
-        // ---- running max / sum over the valid keys of this chunk
-        float cm_lo = -INFINITY, cm_hi = -INFINITY;
+        if (MODE == LONG_FUSED) {
+          // ---- running max / sum over the valid keys of this chunk
+          float cm_lo = -INFINITY, cm_hi = -INFINITY;
 #pragma unroll
-        for (int nt = 0; nt < NTC; ++nt)
+          for (int nt = 0; nt < NTC; ++nt)
 #pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const int col = nt * 8 + 2 * t + (i & 1);
-            if (col < ncols) { if (i < 2) cm_lo = fmaxf(cm_lo, acc[nt][i]); else cm_hi = fmaxf(cm_hi, acc[nt][i]); }
-          }
-        cm_lo = fmaxf(cm_lo, __shfl_xor_sync(0xffffffffu, cm_lo, 1));
-        cm_lo = fmaxf(cm_lo, __shfl_xor_sync(0xffffffffu, cm_lo, 2));
-        cm_hi = fmaxf(cm_hi, __shfl_xor_sync(0xffffffffu, cm_hi, 1));
-        cm_hi = fmaxf(cm_hi, __shfl_xor_sync(0xffffffffu, cm_hi, 2));
-        const float mn_lo = fmaxf(m_lo, cm_lo), mn_hi = fmaxf(m_hi, cm_hi);
-        // exp(-inf - finite) = 0 on the first chunk; a row of all -inf keeps m = -inf and l = NaN -> pattern 0 below, as the reference
-        l_lo *= (m_lo == mn_lo) ? 1.f : (BF ? __expf(m_lo - mn_lo) : expf(m_lo - mn_lo));
-        l_hi *= (m_hi == mn_hi) ? 1.f : (BF ? __expf(m_hi - mn_hi) : expf(m_hi - mn_hi));
-        m_lo = mn_lo; m_hi = mn_hi;
-#pragma unroll
-        for (int nt = 0; nt < NTC; ++nt)
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const int col = nt * 8 + 2 * t + (i & 1);
-            if (col < ncols) {
-              const float x = acc[nt][i] - (i < 2 ? m_lo : m_hi);
-              const float e = BF ? __expf(x) : expf(x);
-              if (i < 2) l_lo += e; else l_hi += e;
+            for (int i = 0; i < 4; ++i) {
+              const int col = nt * 8 + 2 * t + (i & 1);
+              if (col < ncols) { if (i < 2) cm_lo = fmaxf(cm_lo, acc[nt][i]); else cm_hi = fmaxf(cm_hi, acc[nt][i]); }
             }
-          }
+          cm_lo = fmaxf(cm_lo, __shfl_xor_sync(0xffffffffu, cm_lo, 1));
+          cm_lo = fmaxf(cm_lo, __shfl_xor_sync(0xffffffffu, cm_lo, 2));
+          cm_hi = fmaxf(cm_hi, __shfl_xor_sync(0xffffffffu, cm_hi, 1));
+          cm_hi = fmaxf(cm_hi, __shfl_xor_sync(0xffffffffu, cm_hi, 2));
+          const float mn_lo = fmaxf(m_lo, cm_lo), mn_hi = fmaxf(m_hi, cm_hi);
+          // exp(-inf - finite) = 0 on the first chunk; a row of all -inf keeps m = -inf and l = NaN -> pattern 0 below, as the reference
+          l_lo *= (m_lo == mn_lo) ? 1.f : (BF ? __expf(m_lo - mn_lo) : expf(m_lo - mn_lo));
+          l_hi *= (m_hi == mn_hi) ? 1.f : (BF ? __expf(m_hi - mn_hi) : expf(m_hi - mn_hi));
+          m_lo = mn_lo; m_hi = mn_hi;
+#pragma unroll
+          for (int nt = 0; nt < NTC; ++nt)
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+              const int col = nt * 8 + 2 * t + (i & 1);
+              if (col < ncols) {
+                const float x = acc[nt][i] - (i < 2 ? m_lo : m_hi);
+                const float e = BF ? __expf(x) : expf(x);
+                if (i < 2) l_lo += e; else l_hi += e;
+              }
+            }
+        }
         if (scores) {
 #pragma unroll
           for (int nt = 0; nt < NTC; ++nt) {
@@ -233,33 +275,35 @@ __global__ void __launch_bounds__(NW * 32) k_attention_long(const T* __restrict_
           __syncwarp();
         }
       } else {
-        if (c == 0) {                                        // finish pass 1: per-row sum over the quad, one divide per row
-          l_lo += __shfl_xor_sync(0xffffffffu, l_lo, 1);
-          l_lo += __shfl_xor_sync(0xffffffffu, l_lo, 2);
-          l_hi += __shfl_xor_sync(0xffffffffu, l_hi, 1);
-          l_hi += __shfl_xor_sync(0xffffffffu, l_hi, 2);
-          inv_lo = 1.f / l_lo; inv_hi = 1.f / l_hi;
-        }
-        // ---- P chunk = round(exp(S - m) / l), NaN -> 0 (attention.py:149), keys past T -> 0
-#pragma unroll
-        for (int nt = 0; nt < NTC; ++nt)
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const int col = nt * 8 + 2 * t + (i & 1);
-            const float x = acc[nt][i] - (i < 2 ? m_lo : m_hi);
-            float p = (BF ? __expf(x) : expf(x)) * (i < 2 ? inv_lo : inv_hi);
-            if (isnan(p)) p = 0.f;
-            acc[nt][i] = col < ncols ? round_to<T>(p) : 0.f;
+        if (MODE == LONG_FUSED) {
+          if (c == 0) {                                        // finish pass 1: per-row sum over the quad, one divide per row
+            l_lo += __shfl_xor_sync(0xffffffffu, l_lo, 1);
+            l_lo += __shfl_xor_sync(0xffffffffu, l_lo, 2);
+            l_hi += __shfl_xor_sync(0xffffffffu, l_hi, 1);
+            l_hi += __shfl_xor_sync(0xffffffffu, l_hi, 2);
+            inv_lo = 1.f / l_lo; inv_hi = 1.f / l_hi;
           }
-        if (pattern) {
+          // ---- P chunk = round(exp(S - m) / l), NaN -> 0 (attention.py:149), keys past T -> 0
 #pragma unroll
-          for (int nt = 0; nt < NTC; ++nt) {
-            stage_put(stage + g * KC + nt * 8 + 2 * t, acc[nt][0], acc[nt][1]);
-            stage_put(stage + (g + 8) * KC + nt * 8 + 2 * t, acc[nt][2], acc[nt][3]);
+          for (int nt = 0; nt < NTC; ++nt)
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+              const int col = nt * 8 + 2 * t + (i & 1);
+              const float x = acc[nt][i] - (i < 2 ? m_lo : m_hi);
+              float p = (BF ? __expf(x) : expf(x)) * (i < 2 ? inv_lo : inv_hi);
+              if (isnan(p)) p = 0.f;
+              acc[nt][i] = col < ncols ? round_to<T>(p) : 0.f;
+            }
+          if (pattern) {
+#pragma unroll
+            for (int nt = 0; nt < NTC; ++nt) {
+              stage_put(stage + g * KC + nt * 8 + 2 * t, acc[nt][0], acc[nt][1]);
+              stage_put(stage + (g + 8) * KC + nt * 8 + 2 * t, acc[nt][2], acc[nt][3]);
+            }
+            __syncwarp();
+            copy_rows_out<T>(pattern + sc_row0 * Tn + kc0, Tn, stage, nvalid, ncols, lane);
+            __syncwarp();
           }
-          __syncwarp();
-          copy_rows_out<T>(pattern + sc_row0 * Tn + kc0, Tn, stage, nvalid, ncols, lane);
-          __syncwarp();
         }
         // ---- Z += P_chunk V_chunk
         if constexpr (BF) {
@@ -294,25 +338,27 @@ __global__ void __launch_bounds__(NW * 32) k_attention_long(const T* __restrict_
       }
     }
   }
-  if (!active) return;
-  // ---- z rows: [16][DH] through the stage, 16-byte vectors per token row
+  if constexpr (MODE != LONG_SCORES) {
+    if (!active) return;
+    // ---- z rows: [16][DH] through the stage, 16-byte vectors per token row
 #pragma unroll
-  for (int nn = 0; nn < DH / 8; ++nn) {
-    stage_put(stage + g * KC + nn * 8 + 2 * t, o[nn][0], o[nn][1]);
-    stage_put(stage + (g + 8) * KC + nn * 8 + 2 * t, o[nn][2], o[nn][3]);
-  }
-  __syncwarp();
-  for (int i = lane; i < nvalid * VPR; i += 32) {
-    const int r = i / VPR, e = (i % VPR) * VEC;
-    *reinterpret_cast<uint4*>(z + head_base + (int64_t)(wrow0 + r) * tok_stride + e) = *reinterpret_cast<const uint4*>(stage + r * KC + e);
+    for (int nn = 0; nn < DH / 8; ++nn) {
+      stage_put(stage + g * KC + nn * 8 + 2 * t, o[nn][0], o[nn][1]);
+      stage_put(stage + (g + 8) * KC + nn * 8 + 2 * t, o[nn][2], o[nn][3]);
+    }
+    __syncwarp();
+    for (int i = lane; i < nvalid * VPR; i += 32) {
+      const int r = i / VPR, e = (i % VPR) * VEC;
+      *reinterpret_cast<uint4*>(z + head_base + (int64_t)(wrow0 + r) * tok_stride + e) = *reinterpret_cast<const uint4*>(stage + r * KC + e);
+    }
   }
 }
 
-template <typename T>
+template <typename T, int MODE>
 int launch_long(const PbAttention* p, cudaStream_t st) {
   constexpr int NW = 4;
   const size_t smem = ((size_t)(NW * 16 + 2 * KC) * Lay<T>::LD + (size_t)NW * 16 * KC) * sizeof(T);
-  auto kern = k_attention_long<T, NW>;
+  auto kern = k_attention_long<T, NW, MODE>;
   static bool attr_done = false;
   if (!attr_done && smem > 48 * 1024) {
     PB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -334,5 +380,18 @@ int launch_long(const PbAttention* p, cudaStream_t st) {
 int pb_attention_long(const PbAttention* p, cudaStream_t st) {
   if (p->dh != DH) return PB_EUNSUPPORTED;
   if (((uintptr_t)p->q | (uintptr_t)p->k | (uintptr_t)p->v | (uintptr_t)p->z) & 15) return PB_EUNSUPPORTED;
-  return p->dtype == PB_F32 ? launch_long<float>(p, st) : launch_long<bf16>(p, st);
+  return p->dtype == PB_F32 ? launch_long<float, LONG_FUSED>(p, st) : launch_long<bf16, LONG_FUSED>(p, st);
+}
+
+// The split stages for d_head == 64 (attention.cu routes T > 608 here): q, k -> scores and pattern, v -> z.
+// PB_EUNSUPPORTED when d_head != 64 or the q / k (scores) or v / z (pv) pointers are not 16-byte aligned.
+int pb_attn_scores_long(const PbAttention* p, cudaStream_t st) {
+  if (p->dh != DH) return PB_EUNSUPPORTED;
+  if (((uintptr_t)p->q | (uintptr_t)p->k) & 15) return PB_EUNSUPPORTED;
+  return p->dtype == PB_F32 ? launch_long<float, LONG_SCORES>(p, st) : launch_long<bf16, LONG_SCORES>(p, st);
+}
+int pb_attn_pv_long(const PbAttention* p, cudaStream_t st) {
+  if (p->dh != DH) return PB_EUNSUPPORTED;
+  if (((uintptr_t)p->v | (uintptr_t)p->z) & 15) return PB_EUNSUPPORTED;
+  return p->dtype == PB_F32 ? launch_long<float, LONG_PV>(p, st) : launch_long<bf16, LONG_PV>(p, st);
 }

@@ -258,25 +258,29 @@ extern "C" int pb_mean_tokens(const void* x, void* out, int32_t B, int32_t Tn, i
 }
 
 // ------------------------------------------------------------------ im2col
-// patches[(b*np + py*g + px), (c*P + i)*P + j] = images[b, c, py*P + i, px*P + j]
+// Tubelets of D frames x P x P pixels (nt = F / D tubelets in time, g = S / P patches per side); images are F = D = 1:
+//   patches[((b*nt + t)*g + py)*g + px, ((c*D + dt)*P + i)*P + j] = x[b, c, t*D + dt, py*P + i, px*P + j]
+// Frames past nt*D are not read, as Conv3d with stride D drops them.
 // One thread moves VEC contiguous pixels of one patch row (j..j+VEC-1): reads and writes are both
 // contiguous runs of P elements, so with P % 4 == 0 every access is a 16 B (fp32) / 8 B (bf16) vector.
 template <typename T, int VEC>
-__global__ void __launch_bounds__(256) k_im2col(const T* __restrict__ img, T* __restrict__ out, int B, int C, int S, int P) {
-  const int g = S / P;
-  const int pv = P / VEC;                                 // vectors per patch row
-  const int64_t total = (int64_t)B * g * g * C * P * pv;  // one item = one vector
+__global__ void __launch_bounds__(256) k_im2col(const T* __restrict__ img, T* __restrict__ out, int B, int C, int F, int S, int P, int D) {
+  const int g = S / P, nt = F / D;
+  const int pv = P / VEC;                                          // vectors per patch row
+  const int64_t total = (int64_t)B * nt * g * g * C * D * P * pv;  // one item = one vector
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   for (int64_t it = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; it < total; it += stride) {
     int64_t r = it;
     const int jv = (int)(r % pv); r /= pv;
     const int i = (int)(r % P);   r /= P;
+    const int dt = (int)(r % D);  r /= D;
     const int c = (int)(r % C);   r /= C;
     const int px = (int)(r % g);  r /= g;
     const int py = (int)(r % g);  r /= g;
+    const int t = (int)(r % nt);  r /= nt;
     const int b = (int)r;
-    const T* src = img + (((int64_t)b * C + c) * S + (py * P + i)) * S + px * P + jv * VEC;
-    T* dst = out + (((int64_t)b * g + py) * g + px) * ((int64_t)C * P * P) + ((int64_t)c * P + i) * P + jv * VEC;
+    const T* src = img + ((((int64_t)b * C + c) * F + (t * D + dt)) * S + (py * P + i)) * S + px * P + jv * VEC;
+    T* dst = out + ((((int64_t)b * nt + t) * g + py) * g + px) * ((int64_t)C * D * P * P) + (((int64_t)c * D + dt) * P + i) * P + jv * VEC;
     if (VEC == 4) {
       float v[4];
       ld4(src, v);
@@ -286,23 +290,33 @@ __global__ void __launch_bounds__(256) k_im2col(const T* __restrict__ img, T* __
     }
   }
 }
-extern "C" int pb_im2col_patches(const void* images, void* patches, int32_t B, int32_t C, int32_t S, int32_t P, int32_t dtype, pb_stream_t s) {
-  PB_CHECK_ARG(images && patches && B >= 0 && C > 0 && S > 0 && P > 0 && S % P == 0, "pb_im2col_patches: bad geometry (S=%d P=%d)", S, P);
+static int launch_im2col(const void* images, void* patches, int B, int C, int F, int S, int P, int D, int dtype, pb_stream_t s) {
   if (B == 0) return PB_OK;
   const bool vec = (P % 4 == 0) && (S % 4 == 0) && (((uintptr_t)images | (uintptr_t)patches) & 15) == 0;
   const int g = S / P;
-  int64_t items = (int64_t)B * g * g * C * P * (vec ? P / 4 : P);
+  int64_t items = (int64_t)B * (F / D) * g * g * C * D * P * (vec ? P / 4 : P);
   int grid = stream_grid(items, 256);
   cudaStream_t st = (cudaStream_t)s;
   if (dtype == PB_F32) {
-    if (vec) k_im2col<float, 4><<<grid, 256, 0, st>>>((const float*)images, (float*)patches, B, C, S, P);
-    else k_im2col<float, 1><<<grid, 256, 0, st>>>((const float*)images, (float*)patches, B, C, S, P);
+    if (vec) k_im2col<float, 4><<<grid, 256, 0, st>>>((const float*)images, (float*)patches, B, C, F, S, P, D);
+    else k_im2col<float, 1><<<grid, 256, 0, st>>>((const float*)images, (float*)patches, B, C, F, S, P, D);
   } else if (dtype == PB_BF16) {
-    if (vec) k_im2col<bf16, 4><<<grid, 256, 0, st>>>((const bf16*)images, (bf16*)patches, B, C, S, P);
-    else k_im2col<bf16, 1><<<grid, 256, 0, st>>>((const bf16*)images, (bf16*)patches, B, C, S, P);
-  } else PB_CHECK_ARG(false, "pb_im2col_patches: unknown dtype %d", dtype);
+    if (vec) k_im2col<bf16, 4><<<grid, 256, 0, st>>>((const bf16*)images, (bf16*)patches, B, C, F, S, P, D);
+    else k_im2col<bf16, 1><<<grid, 256, 0, st>>>((const bf16*)images, (bf16*)patches, B, C, F, S, P, D);
+  } else PB_CHECK_ARG(false, "pb_im2col: unknown dtype %d", dtype);
   PB_LAUNCH_CHECK();
   return PB_OK;
+}
+extern "C" int pb_im2col_patches(const void* images, void* patches, int32_t B, int32_t C, int32_t S, int32_t P, int32_t dtype, pb_stream_t s) {
+  PB_CHECK_ARG(images && patches && B >= 0 && C > 0 && S > 0 && P > 0 && S % P == 0, "pb_im2col_patches: bad geometry (S=%d P=%d)", S, P);
+  return launch_im2col(images, patches, B, C, 1, S, P, 1, dtype, s);
+}
+// video tubelets (reference models/layers/patch_embedding.py:36-62, Conv3d with kernel = stride = (D, P, P))
+extern "C" int pb_im2col_tubelets(const void* images, void* patches, int32_t B, int32_t C, int32_t F, int32_t S, int32_t P, int32_t D,
+                                  int32_t dtype, pb_stream_t s) {
+  PB_CHECK_ARG(images && patches && B >= 0 && C > 0 && S > 0 && P > 0 && S % P == 0 && D > 0 && F >= D,
+               "pb_im2col_tubelets: bad geometry (F=%d D=%d S=%d P=%d)", F, D, S, P);
+  return launch_im2col(images, patches, B, C, F, S, P, D, dtype, s);
 }
 
 // ---------------------------------------------------------- embed assemble

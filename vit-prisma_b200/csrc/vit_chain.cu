@@ -59,14 +59,24 @@ extern "C" int pb_vit_forward(const PbVitForward* f, pb_stream_t stream) {
   const int64_t M64 = (int64_t)B * T;
   PB_CHECK_ARG(M64 < (1ll << 31), "pb_vit_forward: batch*tokens overflows int32");
   const int M = (int)M64;
-  const int CPP = f->n_channels * f->patch_size * f->patch_size;
+  PB_CHECK_ARG(f->tubelet_depth >= 0, "pb_vit_forward: tubelet_depth %d < 0", f->tubelet_depth);
+  const int D = f->tubelet_depth > 0 ? f->tubelet_depth : 1;     // video: tubelets of D frames; image: one frame
+  if (f->tubelet_depth > 0) {
+    const int g = f->patch_size > 0 ? f->image_size / f->patch_size : 0;
+    PB_CHECK_ARG(f->n_frames >= D && f->n_patches == g * g * (f->n_frames / D),
+                 "pb_vit_forward: n_patches %d != (S/P)^2 * (n_frames %d / tubelet_depth %d)", f->n_patches, f->n_frames, D);
+  }
+  const int CPP = f->n_channels * D * f->patch_size * f->patch_size;   // patch GEMM K
   const bool x3 = f->dtype == PB_F32 && f->gemm_impl != PB_GEMM_SIMT && f->lo_scratch != nullptr;
   float* lo_a = f->lo_scratch;                                   // [M, d] or [M, HD] or patches
   float* lo_b = f->lo_scratch ? f->lo_scratch + (int64_t)M * d : nullptr;  // [M, max(dm, HD)]
   PbGemm g;
 
-  // ---- patch embedding: im2col + GEMM (+bias) -> hook_embed; cls/pos assembly -> hook_full_embed
-  PB_TRY(pb_im2col_patches(f->images, f->patches, B, f->n_channels, f->image_size, f->patch_size, f->dtype, stream));
+  // ---- patch (or tubelet) embedding: im2col + GEMM (+bias) -> hook_embed; cls/pos assembly -> hook_full_embed
+  if (f->tubelet_depth > 0)
+    PB_TRY(pb_im2col_tubelets(f->images, f->patches, B, f->n_channels, f->n_frames, f->image_size, f->patch_size, D, f->dtype, stream));
+  else
+    PB_TRY(pb_im2col_patches(f->images, f->patches, B, f->n_channels, f->image_size, f->patch_size, f->dtype, stream));
   gemm_init(&g, f, B * f->n_patches, d, CPP);
   g.A = f->patches; g.B = f->patch_w; g.bias = f->patch_b; g.out0 = f->embed;
   if (x3 && f->patch_w_lo) {

@@ -81,6 +81,7 @@ class PbVitForward(C.Structure):
         + [("spills_host", C.POINTER(PbVitLayerSpill))]
         + [(n, vp) for n in (
             "lnf_scale", "lnf_norm_f32", "lnf_out", "pooled", "pre_normalize", "out", "lo_scratch")]
+        + [("n_frames", i32), ("tubelet_depth", i32)]
     )
 
 
@@ -107,6 +108,7 @@ SIGNATURES = {
     "pb_l2_normalize_rows": (i32, [vp, vp, i64, i32, f32, i32, vp]),
     "pb_mean_tokens": (i32, [vp, vp, i32, i32, i32, i32, vp]),
     "pb_im2col_patches": (i32, [vp, vp, i32, i32, i32, i32, i32, vp]),
+    "pb_im2col_tubelets": (i32, [vp, vp, i32, i32, i32, i32, i32, i32, i32, vp]),
     "pb_embed_assemble": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, i32, vp]),
     "pb_cast": (i32, [vp, i32, vp, i32, i64, vp]),
     "pb_vit_forward": (i32, [C.POINTER(PbVitForward), vp]),

@@ -276,6 +276,20 @@ def im2col_patches(images: torch.Tensor, patch: int) -> torch.Tensor:
     return out
 
 
+def im2col_tubelets(videos: torch.Tensor, patch: int, depth: int) -> torch.Tensor:
+    """[B, C, F, S, S] -> [B * (F // depth) * (S // patch)^2, C * depth * patch^2], tokens ordered (t, h, w) with t slowest;
+    frames past (F // depth) * depth are dropped, as ``Conv3d`` with stride ``depth`` drops them."""
+    _need_cuda(videos)
+    videos = videos.contiguous()
+    B, Cc, F, S, S2 = videos.shape
+    assert S == S2, "square frames only"
+    g, nt = S // patch, F // depth
+    out = torch.empty((B * nt * g * g, Cc * depth * patch * patch), dtype=videos.dtype, device=videos.device)
+    L.check(L.get_lib().pb_im2col_tubelets(videos.data_ptr(), out.data_ptr(), B, Cc, F, S, patch, depth, dtype_code(videos.dtype),
+                                           _stream()), "pb_im2col_tubelets")
+    return out
+
+
 def cast(x: torch.Tensor, dtype: torch.dtype) -> torch.Tensor:
     _need_cuda(x)
     if x.dtype == dtype:

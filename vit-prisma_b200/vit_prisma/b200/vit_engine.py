@@ -63,12 +63,13 @@ class _Arena:
 def fusable_reason(model, x: torch.Tensor) -> Optional[str]:
     """None when the fused chain can serve ``model(x)``; else a human-readable reason."""
     cfg = model.cfg
-    if not (isinstance(x, torch.Tensor) and x.is_cuda and x.dim() == 4):
-        return "input is not a CUDA [B,C,H,W] tensor"
+    video = cfg.is_video_transformer
+    if not (isinstance(x, torch.Tensor) and x.is_cuda and x.dim() == (5 if video else 4)):
+        return "input is not a CUDA [B,C,F,H,W] tensor" if video else "input is not a CUDA [B,C,H,W] tensor"
     if cfg.dtype not in (torch.float32, torch.bfloat16):
         return f"dtype {cfg.dtype}"
-    if cfg.is_video_transformer or cfg.use_bert_block or cfg.attn_only:
-        return "video / bert / attn-only architecture"
+    if cfg.use_bert_block or cfg.attn_only:
+        return "bert / attn-only architecture"
     if cfg.normalization_type not in ("LN", "LNPre"):
         return "normalization_type is not LN/LNPre"
     if cfg.activation_name not in activation_fns.ELEMENTWISE:
@@ -81,8 +82,10 @@ def fusable_reason(model, x: torch.Tensor) -> Optional[str]:
         pass  # x[:, 0] is still well defined
     if model.training and (cfg.attn_dropout_rate > 0 or cfg.mlp_dropout_rate > 0):
         return "dropout active"
-    if x.shape[1] != cfg.n_channels or x.shape[2] != cfg.image_size or x.shape[3] != cfg.image_size:
+    if x.shape[1] != cfg.n_channels or x.shape[-2] != cfg.image_size or x.shape[-1] != cfg.image_size:
         return "image geometry differs from cfg"
+    if video and x.shape[2] // cfg.video_tubelet_depth != cfg.video_num_frames // cfg.video_tubelet_depth:
+        return "number of tubelets differs from cfg (W_pos would not match)"
     if model.cls_token.device != x.device:
         return "model and input on different devices"
     if torch.is_grad_enabled() and any(p.requires_grad for p in (model.cls_token,)) and x.requires_grad:
@@ -177,8 +180,10 @@ class VitEngine:
             return None
 
         plan: Dict[str, object] = {}
+        depth = cfg.video_tubelet_depth if cfg.is_video_transformer else 1
+        K_patch = cfg.n_channels * depth * cfg.patch_size ** 2          # patch GEMM K: C*D*P*P (D = 1 for images)
         plan["patches"] = ("s", "patches")
-        tmp["patches"] = scratch.reserve((B * NP, cfg.n_channels * cfg.patch_size ** 2), dt)
+        tmp["patches"] = scratch.reserve((B * NP, K_patch), dt)
         plan["embed"] = place("hook_embed", (B, NP, d), dt, True)
         plan["full_embed"] = place("hook_full_embed", (B, T, d), dt, True)
         if cfg.layer_norm_pre:
@@ -257,7 +262,7 @@ class VitEngine:
 
         x3 = fp32 and gemm_impl != L.GEMM_SIMT
         if x3:
-            lo_elems = max(B * T * (d + max(dm, HD)), B * NP * cfg.n_channels * cfg.patch_size ** 2)
+            lo_elems = max(B * T * (d + max(dm, HD)), B * NP * K_patch)
             tmp["lo"] = scratch.reserve((lo_elems,), torch.float32)
 
         arena.commit()
@@ -281,6 +286,8 @@ class VitEngine:
         f.eps = float(cfg.eps)
         f.attn_scale = float(m.blocks[0].attn.attn_scale) if cfg.n_layers else 1.0
         f.images = x.data_ptr()
+        if cfg.is_video_transformer:
+            f.n_frames, f.tubelet_depth = x.shape[2], depth
         f.patch_w, f.patch_b = patch_w.data_ptr(), m.embed.proj.bias.data_ptr()
         f.patch_w_lo = patch_w_lo.data_ptr() if patch_w_lo is not None else None
         f.cls, f.pos = m.cls_token.data_ptr(), m.pos_embed.W_pos.data_ptr()

@@ -115,7 +115,7 @@ _FIELDS = [
     ("save_dir", str, "Checkpoints"),
     ("save_checkpoints", bool, True),
     ("save_cp_frequency", int, 5),
-    # video (tubelet) towers: accepted, not on the H100 hot path
+    # video (tubelet) towers: input [B, C, video_num_frames, S, S], tubelets of video_tubelet_depth frames x P x P
     ("is_video_transformer", bool, False),
     ("video_tubelet_depth", Optional[int], None),
     ("video_num_frames", Optional[int], None),
@@ -127,7 +127,10 @@ def _from_dict(cls, config_dict: Dict[str, Any]):
 
 
 def _n_patches(self) -> int:
-    return (self.image_size // self.patch_size) ** 2
+    n = (self.image_size // self.patch_size) ** 2
+    if self.is_video_transformer:
+        n *= self.video_num_frames // self.video_tubelet_depth
+    return n
 
 
 def _n_tokens(self) -> int:

@@ -42,8 +42,11 @@ class PatchEmbedding(nn.Module):
 
 
 class TubeletEmbedding(nn.Module):
-    """Video tubelet embedding (reference :36-62).  Parameter container only: the H100 hot path covers
-    image towers; calling it raises instead of silently running somewhere else."""
+    """Video tubelet embedding (reference :36-62): ``nn.Conv3d(C, d, kernel=stride=(D, P, P))`` over ``[B, C, F, S, S]``.
+    With stride == kernel it is the same GEMM as the 2-D case: tubelet im2col -> [B*n_tubelets, C*D*P*P] @
+    proj.weight.view(d, C*D*P*P)^T + bias, tokens ordered (t, h, w) with t slowest.  Frames past (F // D) * D are
+    dropped, as Conv3d drops them.  ``self.proj`` stays an ``nn.Conv3d`` as the parameter container
+    (``embed.proj.weight [d, C, D, P, P]``)."""
 
     def __init__(self, cfg):
         super().__init__()
@@ -52,5 +55,11 @@ class TubeletEmbedding(nn.Module):
         self.proj = nn.Conv3d(cfg.n_channels, cfg.d_model, kernel_size=size, stride=size, bias=True)
 
     @host_staged
-    def forward(self, x):
-        raise NotImplementedError("TubeletEmbedding (video) is outside the H100 hot-path scope (SURVEY #6)")
+    def forward(self, x: torch.Tensor) -> torch.Tensor:
+        B = x.shape[0]
+        D, P, d = self.cfg.video_tubelet_depth, self.cfg.patch_size, self.cfg.d_model
+        w = self.proj.weight
+        x = ops.cast(x, w.dtype) if x.is_cuda else x.to(w.dtype)
+        patches = ops.im2col_tubelets(x, P, D)                   # [B*n_tubelets, C*D*P*P]
+        out, _ = ops.gemm(patches, w.detach().reshape(d, -1), self.proj.bias)
+        return out.view(B, -1, d)                                # [B, n_tubelets, d_model]
