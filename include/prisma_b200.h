@@ -47,7 +47,7 @@ PB_API unsigned long long pb_launch_count(void);
 /* fills sm count / compute capability of the current device; PB_ENODEVICE without a GPU */
 PB_API int pb_device_info(int* sm_count, int* cc_major, int* cc_minor);
 /* sizeof() of the ABI structs as compiled (0 PbGemm, 1 PbLayerNorm, 2 PbAttention, 3 PbVitLayerW,
- * 4 PbVitLayerSpill, 5 PbVitForward, ...; -1 for an unknown index): lets a binding verify its layout */
+ * 4 PbVitLayerSpill, 5 PbVitForward, ..., 10 PbTextForward; -1 for an unknown index): lets a binding verify its layout */
 PB_API int pb_abi_sizeof(int which);
 
 /* ------------------------------------------------------------------- GEMM
@@ -108,12 +108,16 @@ PB_API int pb_layernorm(const PbLayerNorm* p, pb_stream_t stream);
  *   pattern = softmax(scores), NaN -> 0   (hook_pattern;     NULL = not materialised)
  *   z       = pattern v                   (hook_z)
  * pb_attention runs all three in one kernel; the three split entry points exist for the
- * hooked path where user code may edit scores / pattern between the steps.               */
+ * hooked path where user code may edit scores / pattern between the steps.
+ * causal != 0 (pb_attention only; the split stages ignore it): scores[b,h,i,j] = -inf for j > i,
+ * i.e. scores / scale + the additive mask of models/base_text_transformer.py:188-194, so
+ * pattern[b,h,i,j] = 0 there.  Zero-initialised descriptors keep the unmasked behaviour.     */
 typedef struct {
   int32_t B, T, H, dh, dtype;
   float attn_scale;
   const void* q; const void* k; const void* v;
   void* scores; void* pattern; void* z;
+  int32_t causal;
 } PbAttention;
 PB_API int pb_attention(const PbAttention* p, pb_stream_t stream);
 PB_API int pb_attn_scores(const PbAttention* p, pb_stream_t stream);              /* q,k -> scores   */
@@ -144,6 +148,14 @@ PB_API int pb_embed_assemble(const void* embed, const void* cls, const void* pos
                       int32_t B, int32_t n_patches, int32_t d, int32_t use_cls, int32_t dtype,
                       pb_stream_t s);
 PB_API int pb_cast(const void* x, int32_t dtype_in, void* y, int32_t dtype_out, int64_t n, pb_stream_t s);
+/* embed[b,t,:] = W_E[ids[b,t],:]  (nn.Embedding, models/base_text_transformer.py:125) and
+ * full[b,t,:] = embed[b,t,:] + pos[t,:] rounded to dtype (:139-141); ids int64 [B,T], W_E [vocab,d], pos [>=T,d].
+ * Rows whose id lies outside [0, vocab) are filled with NaN and W_E is not read for them (the caller range-checks). */
+PB_API int pb_embed_tokens(const int64_t* ids, const void* W_E, const void* pos, void* embed, void* full,
+                           int32_t B, int32_t T, int32_t d, int32_t vocab, int32_t dtype, pb_stream_t s);
+/* out[b,:] = x[b, argmax_t ids[b,t], :], the first maximal index on ties (base_text_transformer.py:151) */
+PB_API int pb_gather_argmax_rows(const int64_t* ids, const void* x, void* out, int32_t B, int32_t T, int32_t d,
+                                 int32_t dtype, pb_stream_t s);
 
 /* ------------------------------------------------ fused HookedViT forward
  * One call = HookedViT.forward (models/base_vit.py:152-217) with every requested HookPoint
@@ -202,6 +214,34 @@ typedef struct {
   int32_t n_frames, tubelet_depth;
 } PbVitForward;
 PB_API int pb_vit_forward(const PbVitForward* f, pb_stream_t stream);
+
+/* ----------------------------------------------- fused HookedTextTransformer forward
+ * One call = HookedTextTransformer.forward (models/base_text_transformer.py:119-160) with every
+ * requested HookPoint activation spilled, as pb_vit_forward does it: pb_embed_tokens -> the blocks
+ * of pb_vit_forward (same PbVitLayerW / PbVitLayerSpill tables), pb_attention with `causal` ->
+ * ln_final over all tokens -> pb_gather_argmax_rows -> head -> F.normalize.  ln_pre is never
+ * applied, as in the reference.  pos is pos_embed [>= n_tokens, d]; n_tokens may be shorter than
+ * the context only without the causal mask (the reference's [ctx, ctx] mask does not broadcast).   */
+typedef struct {
+  int32_t batch, n_tokens, vocab, d_model, n_heads, d_head, d_mlp, n_classes;
+  int32_t n_layers;
+  int32_t causal;            /* 1: additive -inf mask above the diagonal (build_causal_mask, :188-194) */
+  int32_t normalize_output, head_proj /* return_type != pre_logits */;
+  int32_t act, dtype, gemm_impl;
+  float eps, attn_scale;
+  const int64_t* ids;        /* [B, n_tokens] token ids, all in [0, vocab) */
+  const void *token_w, *pos, *lnf_w, *lnf_b, *head_w, *head_w_lo, *head_b;
+  const PbVitLayerW* layers_host;        /* HOST array [n_layers] */
+  void* embed;               /* hook_embed [B,T,d]                                              */
+  void* full_embed;          /* hook_full_embed == block 0 input [B,T,d]                        */
+  const PbVitLayerSpill* spills_host;    /* HOST array [n_layers] */
+  float* lnf_scale; float* lnf_norm_f32; void* lnf_out;   /* lnf_out [B,T,d] is required          */
+  void* pooled;              /* [B,d] ln_final row at each row's end-of-text position           */
+  void* pre_normalize;       /* hook_post_head_pre_normalize [B, n_classes or d]                */
+  void* out;                 /* model output                                                    */
+  float* lo_scratch;         /* fp32 [B*T*(d + max(d_mlp, H*dh))] for 3xTF32 GEMMs, or NULL       */
+} PbTextForward;
+PB_API int pb_text_forward(const PbTextForward* f, pb_stream_t stream);
 
 /* ------------------------------------------------------- TopK SAE training step
  * Stands in for StandardSparseAutoencoder.forward + VisionSAETrainer.train_step

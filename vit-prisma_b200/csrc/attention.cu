@@ -24,7 +24,8 @@ int pb_attn_pv_long(const PbAttention* p, cudaStream_t st);
 
 enum { ATT_FUSED = 0, ATT_SCORES = 1, ATT_PV = 2 };
 
-template <typename T, int KPL, int EPL, int MODE>
+// CAUSAL (ATT_FUSED only): keys j > query i score -inf, as scores / scale + mask does; they drop out of the max and get e = 0
+template <typename T, int KPL, int EPL, int MODE, bool CAUSAL>
 __global__ void __launch_bounds__(256) k_attention(const T* __restrict__ q, const T* __restrict__ k, const T* __restrict__ v,
                                                    T* __restrict__ scores, T* __restrict__ pattern, T* __restrict__ z, int B, int Tn,
                                                    int H, int dh, float attn_scale, int rows_per_cta) {
@@ -98,7 +99,8 @@ __global__ void __launch_bounds__(256) k_attention(const T* __restrict__ q, cons
           for (int m = 0; m < KPL; ++m) {
             const int j = m * 32 + lane;
             if (j < Tn) {
-              const float s = round_to<T>(round_to<T>(acc[m][r]) / attn_scale);  // einsum -> tensor, then "/ attn_scale" -> tensor
+              float s = round_to<T>(round_to<T>(acc[m][r]) / attn_scale);  // einsum -> tensor, then "/ attn_scale" -> tensor
+              if (CAUSAL && j > r0 + r) s = -INFINITY;
               acc[m][r] = s;
               if (scores) st_from_float(scores + ob + j, s);
               mx = fmaxf(mx, s);
@@ -178,7 +180,7 @@ __global__ void __launch_bounds__(256) k_attention(const T* __restrict__ q, cons
   }
 }
 
-template <typename T, int KPL, int EPL, int MODE>
+template <typename T, int KPL, int EPL, int MODE, bool CAUSAL>
 static int launch_att_inst(const PbAttention* p, cudaStream_t st) {
   const int TP = KPL * 32;
   const int threads = p->T <= 64 ? 128 : 256;
@@ -190,7 +192,7 @@ static int launch_att_inst(const PbAttention* p, cudaStream_t st) {
     pb_set_error("pb_attention: T=%d dh=%d needs %zu B of shared memory (> 227 KB); sequence too long for this kernel", p->T, p->dh, smem);
     return PB_EUNSUPPORTED;
   }
-  auto kern = k_attention<T, KPL, EPL, MODE>;
+  auto kern = k_attention<T, KPL, EPL, MODE, CAUSAL>;
   if (smem > 48 * 1024) PB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   dim3 grid(p->B * p->H, (p->T + rows_per_cta - 1) / rows_per_cta);
   kern<<<grid, threads, smem, st>>>((const T*)p->q, (const T*)p->k, (const T*)p->v, (T*)p->scores, (T*)p->pattern, (T*)p->z, p->B, p->T,
@@ -199,14 +201,14 @@ static int launch_att_inst(const PbAttention* p, cudaStream_t st) {
   return PB_OK;
 }
 
-template <typename T, int MODE>
+template <typename T, int MODE, bool CAUSAL = false>
 static int launch_att(const PbAttention* p, cudaStream_t st) {
   const int kpl = (p->T + 31) / 32, epl = (p->dh + 31) / 32;
 #define PB_ATT_E(KPL)                                                                       \
   do {                                                                                      \
-    if (epl <= 1) return launch_att_inst<T, KPL, 1, MODE>(p, st);                           \
-    if (epl <= 2) return launch_att_inst<T, KPL, 2, MODE>(p, st);                           \
-    if (epl <= 4) return launch_att_inst<T, KPL, 4, MODE>(p, st);                           \
+    if (epl <= 1) return launch_att_inst<T, KPL, 1, MODE, CAUSAL>(p, st);                   \
+    if (epl <= 2) return launch_att_inst<T, KPL, 2, MODE, CAUSAL>(p, st);                   \
+    if (epl <= 4) return launch_att_inst<T, KPL, 4, MODE, CAUSAL>(p, st);                   \
   } while (0)
   if (epl > 4) { pb_set_error("pb_attention: d_head=%d > 128 unsupported", p->dh); return PB_EUNSUPPORTED; }
   if (kpl <= 1) PB_ATT_E(1);
@@ -253,7 +255,9 @@ extern "C" int pb_attention(const PbAttention* p, pb_stream_t stream) {
       if (rc != PB_EUNSUPPORTED) return rc;
     }
   }
-  return p->dtype == PB_F32 ? launch_att<float, ATT_FUSED>(p, (cudaStream_t)stream) : launch_att<bf16, ATT_FUSED>(p, (cudaStream_t)stream);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (p->causal) return p->dtype == PB_F32 ? launch_att<float, ATT_FUSED, true>(p, st) : launch_att<bf16, ATT_FUSED, true>(p, st);
+  return p->dtype == PB_F32 ? launch_att<float, ATT_FUSED>(p, st) : launch_att<bf16, ATT_FUSED>(p, st);
 }
 extern "C" int pb_attn_scores(const PbAttention* p, pb_stream_t stream) {
   PB_TRY(check_att(p, "pb_attn_scores"));

@@ -15,6 +15,11 @@
 //   LONG_PV:     pass 2 with P read from a [B,H,T,T] pattern in 64-key chunks instead of computed -> z.
 // Both share the fused mode's arithmetic and rounding points, so the scores equal the fused kernel's scores spill bit for bit, and
 // the z of LONG_PV fed the fused kernel's own spilled pattern equals the fused kernel's z bit for bit.
+//
+// CAUSAL (fused mode only, the text towers' mask): keys j > query i score -inf, as scores / scale + mask does.  A CTA's query
+// slab is one 64-row chunk, so key chunks past the slab lie wholly above the diagonal: neither pass loads or multiplies them,
+// and a requested spill gets -inf / 0 there.  Every processed chunk has key kc0 <= each row of the slab, so the running max of
+// a row is finite from chunk 0 on; masked entries are still kept out of the running sum explicitly.
 #include "common.cuh"
 
 namespace {
@@ -95,7 +100,7 @@ __device__ __forceinline__ void copy_rows_in(T* stage, const T* __restrict__ gba
   }
 }
 
-template <typename T, int NW, int MODE>
+template <typename T, int NW, int MODE, bool CAUSAL>
 __global__ void __launch_bounds__(NW * 32) k_attention_long(const T* __restrict__ q, const T* __restrict__ k, const T* __restrict__ v,
                                                            T* __restrict__ scores, T* __restrict__ pattern, T* __restrict__ z, int Tn, int H,
                                                            float attn_scale, float inv_scale) {
@@ -151,7 +156,8 @@ __global__ void __launch_bounds__(NW * 32) k_attention_long(const T* __restrict_
     }
   }
 
-  const int nchunks = (Tn + KC - 1) / KC;
+  // causal: chunks starting past the slab's last query row are all -inf (written below when spilled) and are never loaded
+  const int nchunks = CAUSAL ? min((Tn + KC - 1) / KC, (row0 + NW * 16 - 1) / KC + 1) : (Tn + KC - 1) / KC;
   const int64_t sc_row0 = ((int64_t)b * H + h) * Tn + wrow0;   // first score / pattern row of this warp
   float m_lo = -INFINITY, m_hi = -INFINITY, l_lo = 0.f, l_hi = 0.f;
   float inv_lo = 0.f, inv_hi = 0.f;
@@ -230,6 +236,13 @@ __global__ void __launch_bounds__(NW * 32) k_attention_long(const T* __restrict_
 #pragma unroll
           for (int i = 0; i < 4; ++i) acc[nt][i] = round_to<T>(round_to<T>(acc[nt][i]) / attn_scale);
       }
+      if constexpr (CAUSAL) {
+#pragma unroll
+        for (int nt = 0; nt < NTC; ++nt)
+#pragma unroll
+          for (int i = 0; i < 4; ++i)
+            if (kc0 + nt * 8 + 2 * t + (i & 1) > wrow0 + g + (i < 2 ? 0 : 8)) acc[nt][i] = -INFINITY;
+      }
       const int ncols = min(KC, Tn - kc0);
 
       if (pass == 0) {
@@ -257,7 +270,7 @@ __global__ void __launch_bounds__(NW * 32) k_attention_long(const T* __restrict_
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
               const int col = nt * 8 + 2 * t + (i & 1);
-              if (col < ncols) {
+              if (col < ncols && (!CAUSAL || acc[nt][i] != -INFINITY)) {
                 const float x = acc[nt][i] - (i < 2 ? m_lo : m_hi);
                 const float e = BF ? __expf(x) : expf(x);
                 if (i < 2) l_lo += e; else l_hi += e;
@@ -338,6 +351,18 @@ __global__ void __launch_bounds__(NW * 32) k_attention_long(const T* __restrict_
       }
     }
   }
+  if constexpr (CAUSAL) {                                   // spilled regions of the skipped chunks: scores -inf, pattern 0
+    const int c0 = nchunks * KC;
+    if (active && c0 < Tn) {
+      for (int r = 0; r < nvalid; ++r) {
+        const int64_t rb = (sc_row0 + r) * Tn;
+        for (int j = c0 + lane; j < Tn; j += 32) {
+          if (scores) st_from_float(scores + rb + j, -INFINITY);
+          if (pattern) st_from_float(pattern + rb + j, 0.f);
+        }
+      }
+    }
+  }
   if constexpr (MODE != LONG_SCORES) {
     if (!active) return;
     // ---- z rows: [16][DH] through the stage, 16-byte vectors per token row
@@ -354,11 +379,11 @@ __global__ void __launch_bounds__(NW * 32) k_attention_long(const T* __restrict_
   }
 }
 
-template <typename T, int MODE>
+template <typename T, int MODE, bool CAUSAL = false>
 int launch_long(const PbAttention* p, cudaStream_t st) {
   constexpr int NW = 4;
   const size_t smem = ((size_t)(NW * 16 + 2 * KC) * Lay<T>::LD + (size_t)NW * 16 * KC) * sizeof(T);
-  auto kern = k_attention_long<T, NW, MODE>;
+  auto kern = k_attention_long<T, NW, MODE, CAUSAL>;
   static bool attr_done = false;
   if (!attr_done && smem > 48 * 1024) {
     PB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -380,6 +405,7 @@ int launch_long(const PbAttention* p, cudaStream_t st) {
 int pb_attention_long(const PbAttention* p, cudaStream_t st) {
   if (p->dh != DH) return PB_EUNSUPPORTED;
   if (((uintptr_t)p->q | (uintptr_t)p->k | (uintptr_t)p->v | (uintptr_t)p->z) & 15) return PB_EUNSUPPORTED;
+  if (p->causal) return p->dtype == PB_F32 ? launch_long<float, LONG_FUSED, true>(p, st) : launch_long<bf16, LONG_FUSED, true>(p, st);
   return p->dtype == PB_F32 ? launch_long<float, LONG_FUSED>(p, st) : launch_long<bf16, LONG_FUSED>(p, st);
 }
 

@@ -101,7 +101,8 @@ __device__ __forceinline__ void copy_run(T* __restrict__ g, const T* s, int n_el
   for (int i = done / (int)sizeof(T) + lane; i < n_elems; i += 32) g[i] = s[i];
 }
 
-template <typename T, int NT, int NW>  // NT = key tiles of 8 (TPAD = 8*NT, multiple of 16), NW warps of 16 query rows
+// NT = key tiles of 8 (TPAD = 8*NT, multiple of 16), NW warps of 16 query rows; CAUSAL: keys j > query i score -inf
+template <typename T, int NT, int NW, bool CAUSAL>
 __global__ void __launch_bounds__(NW * 32) k_attention_mma(const T* __restrict__ q, const T* __restrict__ k, const T* __restrict__ v,
                                                           T* __restrict__ scores, T* __restrict__ pattern, T* __restrict__ z, int Tn, int H,
                                                           float attn_scale, float inv_scale, int vb) {
@@ -201,6 +202,13 @@ __global__ void __launch_bounds__(NW * 32) k_attention_mma(const T* __restrict__
     for (int nt = 0; nt < NT; ++nt)
 #pragma unroll
       for (int c = 0; c < 4; ++c) acc[nt][c] = round_to<T>(round_to<T>(acc[nt][c]) / attn_scale);
+  }
+  if constexpr (CAUSAL) {   // scores / scale + mask with mask = -inf above the diagonal: -inf there, out of the max, e = 0
+#pragma unroll
+    for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+      for (int c = 0; c < 4; ++c)
+        if (nt * 8 + 2 * t + (c & 1) > wrow0 + g + (c < 2 ? 0 : 8)) acc[nt][c] = -INFINITY;
   }
   float mx_lo = -INFINITY, mx_hi = -INFINITY;
 #pragma unroll
@@ -322,13 +330,13 @@ int pow2_align(uint64_t x) {   // largest power of two <= 16 dividing x
   return a;
 }
 
-template <typename T, int NT, int NW>
+template <typename T, int NT, int NW, bool CAUSAL>
 int launch_mma(const PbAttention* p, cudaStream_t st) {
   constexpr int TPAD = NT * 8;
   const size_t es = sizeof(T);
   const size_t smem = ((size_t)2 * TPAD * Lay<T>::LD + (size_t)NW * 16 * Lay<T>::LD + (size_t)NW * 16 * TPAD) * es;
   if (smem > 227 * 1024) return PB_EUNSUPPORTED;
-  auto kern = k_attention_mma<T, NT, NW>;
+  auto kern = k_attention_mma<T, NT, NW, CAUSAL>;
   static bool attr_done = false;
   if (!attr_done && smem > 48 * 1024) {
     PB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -350,17 +358,17 @@ int launch_mma(const PbAttention* p, cudaStream_t st) {
   return PB_OK;
 }
 
-template <typename T>
+template <typename T, bool CAUSAL>
 int dispatch_mma(const PbAttention* p, cudaStream_t st) {
-  if (p->T <= 64) return launch_mma<T, 8, 4>(p, st);
-  if (p->T <= 128) return launch_mma<T, 16, 4>(p, st);
+  if (p->T <= 64) return launch_mma<T, 8, 4, CAUSAL>(p, st);
+  if (p->T <= 128) return launch_mma<T, 16, 4, CAUSAL>(p, st);
   // longer rows: K / V streamed in 64-key chunks, two passes (attention_long.cu); PB_ATTN_LONG=0 keeps the whole-row kernels
   // below for cross-checks (T <= 272)
   static int use_long = -1;
   if (use_long < 0) { const char* e = getenv("PB_ATTN_LONG"); use_long = (e && !strcmp(e, "0")) ? 0 : 1; }
   if (use_long) return pb_attention_long(p, st);
-  if (p->T <= 208) return launch_mma<T, 26, 2>(p, st);
-  if (p->T <= 272) return launch_mma<T, 34, 2>(p, st);
+  if (p->T <= 208) return launch_mma<T, 26, 2, CAUSAL>(p, st);
+  if (p->T <= 272) return launch_mma<T, 34, 2, CAUSAL>(p, st);
   return PB_EUNSUPPORTED;
 }
 
@@ -371,5 +379,6 @@ int dispatch_mma(const PbAttention* p, cudaStream_t st) {
 int pb_attention_mma(const PbAttention* p, cudaStream_t st) {
   if (p->dh != DH) return PB_EUNSUPPORTED;
   if (((uintptr_t)p->q | (uintptr_t)p->k | (uintptr_t)p->v | (uintptr_t)p->z) & 15) return PB_EUNSUPPORTED;
-  return p->dtype == PB_F32 ? dispatch_mma<float>(p, st) : dispatch_mma<bf16>(p, st);
+  if (p->causal) return p->dtype == PB_F32 ? dispatch_mma<float, true>(p, st) : dispatch_mma<bf16, true>(p, st);
+  return p->dtype == PB_F32 ? dispatch_mma<float, false>(p, st) : dispatch_mma<bf16, false>(p, st);
 }

@@ -374,3 +374,110 @@ extern "C" int pb_embed_assemble(const void* embed, const void* cls, const void*
   PB_LAUNCH_CHECK();
   return PB_OK;
 }
+
+// ------------------------------------------------------------- text towers
+// embed[b,t,:] = W_E[ids[b,t],:]  (nn.Embedding, base_text_transformer.py:125)
+// full[b,t,:]  = round(embed[b,t,:] + pos[t,:])  (:139-141; pos is pos_embed[:T], broadcast over the batch)
+// One 16-byte vector per thread and step.  Ids outside [0, vocab) are never dereferenced: their rows are filled with NaN
+// (the host checks the range and raises before any launch, as nn.Embedding raises).
+template <typename T, int VEC>
+__global__ void __launch_bounds__(256) k_embed_tokens(const int64_t* __restrict__ ids, const T* __restrict__ W_E, const T* __restrict__ pos,
+                                                      T* __restrict__ embed, T* __restrict__ full, int Tn, int d, int vocab, int64_t total) {
+  const int nv = d / VEC;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t it = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; it < total; it += stride) {
+    const int c = (int)(it % nv) * VEC;
+    const int64_t bt = it / nv;
+    const int t = (int)(bt % Tn);
+    const int64_t id = ids[bt];
+    T e[VEC], f[VEC];
+    if (id >= 0 && id < vocab) {
+      if constexpr (VEC * sizeof(T) == 16) {
+        *reinterpret_cast<uint4*>(e) = *reinterpret_cast<const uint4*>(W_E + id * d + c);
+        uint4 pu = *reinterpret_cast<const uint4*>(pos + (int64_t)t * d + c);
+        const T* p = reinterpret_cast<const T*>(&pu);
+#pragma unroll
+        for (int j = 0; j < VEC; ++j) st_from_float(f + j, ld_as_float(e + j) + ld_as_float(p + j));
+      } else {
+#pragma unroll
+        for (int j = 0; j < VEC; ++j) {
+          e[j] = W_E[id * d + c + j];
+          st_from_float(f + j, ld_as_float(e + j) + ld_as_float(pos + (int64_t)t * d + c + j));
+        }
+      }
+    } else {
+#pragma unroll
+      for (int j = 0; j < VEC; ++j) { st_from_float(e + j, __int_as_float(0x7fc00000)); f[j] = e[j]; }
+    }
+    if constexpr (VEC * sizeof(T) == 16) {
+      *reinterpret_cast<uint4*>(embed + bt * d + c) = *reinterpret_cast<const uint4*>(e);
+      *reinterpret_cast<uint4*>(full + bt * d + c) = *reinterpret_cast<const uint4*>(f);
+    } else {
+#pragma unroll
+      for (int j = 0; j < VEC; ++j) { embed[bt * d + c + j] = e[j]; full[bt * d + c + j] = f[j]; }
+    }
+  }
+}
+extern "C" int pb_embed_tokens(const int64_t* ids, const void* W_E, const void* pos, void* embed, void* full, int32_t B, int32_t T,
+                               int32_t d, int32_t vocab, int32_t dtype, pb_stream_t s) {
+  PB_CHECK_ARG(ids && W_E && pos && embed && full && B >= 0 && T > 0 && d > 0 && vocab > 0, "pb_embed_tokens: bad arguments");
+  PB_CHECK_ARG(dtype == PB_F32 || dtype == PB_BF16, "pb_embed_tokens: unknown dtype %d", dtype);
+  if (B == 0) return PB_OK;
+  const int es = dtype == PB_F32 ? 4 : 2;
+  const bool vec = ((int64_t)d * es) % 16 == 0 && (((uintptr_t)W_E | (uintptr_t)pos | (uintptr_t)embed | (uintptr_t)full) & 15) == 0;
+  const int VEC = vec ? 16 / es : 1;
+  const int64_t total = (int64_t)B * T * (d / VEC);
+  const int grid = stream_grid(total, 256);
+  cudaStream_t st = (cudaStream_t)s;
+  if (dtype == PB_F32) {
+    if (vec) k_embed_tokens<float, 4><<<grid, 256, 0, st>>>(ids, (const float*)W_E, (const float*)pos, (float*)embed, (float*)full, T, d, vocab, total);
+    else k_embed_tokens<float, 1><<<grid, 256, 0, st>>>(ids, (const float*)W_E, (const float*)pos, (float*)embed, (float*)full, T, d, vocab, total);
+  } else {
+    if (vec) k_embed_tokens<bf16, 8><<<grid, 256, 0, st>>>(ids, (const bf16*)W_E, (const bf16*)pos, (bf16*)embed, (bf16*)full, T, d, vocab, total);
+    else k_embed_tokens<bf16, 1><<<grid, 256, 0, st>>>(ids, (const bf16*)W_E, (const bf16*)pos, (bf16*)embed, (bf16*)full, T, d, vocab, total);
+  }
+  PB_LAUNCH_CHECK();
+  return PB_OK;
+}
+
+// out[b,:] = x[b, argmax_t ids[b,t], :] with the first maximal index on ties, as torch.argmax
+// (base_text_transformer.py:151: x[arange(B), input.argmax(-1)]).  One CTA per batch row: a block argmax, then a row copy.
+template <typename T>
+__global__ void __launch_bounds__(256) k_gather_argmax_rows(const int64_t* __restrict__ ids, const T* __restrict__ x, T* __restrict__ out,
+                                                            int Tn, int d) {
+  __shared__ int64_t s_val[8];
+  __shared__ int s_idx[8];
+  const int b = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int64_t* row = ids + (int64_t)b * Tn;
+  int64_t best = INT64_MIN;
+  int bi = INT32_MAX;
+  for (int t = threadIdx.x; t < Tn; t += blockDim.x) {
+    const int64_t v = row[t];
+    if (v > best) { best = v; bi = t; }                     // strided ascending t: first maximum of this thread's share
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const int64_t ov = __shfl_xor_sync(0xffffffffu, best, o);
+    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+    if (ov > best || (ov == best && oi < bi)) { best = ov; bi = oi; }
+  }
+  if (lane == 0) { s_val[warp] = best; s_idx[warp] = bi; }
+  __syncthreads();
+  best = s_val[0]; bi = s_idx[0];
+  for (int w = 1; w < (int)(blockDim.x >> 5); ++w)
+    if (s_val[w] > best || (s_val[w] == best && s_idx[w] < bi)) { best = s_val[w]; bi = s_idx[w]; }
+  const T* src = x + ((int64_t)b * Tn + bi) * d;
+  T* dst = out + (int64_t)b * d;
+  for (int c = threadIdx.x; c < d; c += blockDim.x) dst[c] = src[c];
+}
+extern "C" int pb_gather_argmax_rows(const int64_t* ids, const void* x, void* out, int32_t B, int32_t T, int32_t d, int32_t dtype,
+                                     pb_stream_t s) {
+  PB_CHECK_ARG(ids && x && out && B >= 0 && T > 0 && d > 0, "pb_gather_argmax_rows: bad arguments");
+  if (B == 0) return PB_OK;
+  cudaStream_t st = (cudaStream_t)s;
+  if (dtype == PB_F32) k_gather_argmax_rows<float><<<B, 256, 0, st>>>(ids, (const float*)x, (float*)out, T, d);
+  else if (dtype == PB_BF16) k_gather_argmax_rows<bf16><<<B, 256, 0, st>>>(ids, (const bf16*)x, (bf16*)out, T, d);
+  else PB_CHECK_ARG(false, "pb_gather_argmax_rows: unknown dtype %d", dtype);
+  PB_LAUNCH_CHECK();
+  return PB_OK;
+}

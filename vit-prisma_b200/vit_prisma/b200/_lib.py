@@ -48,6 +48,7 @@ class PbAttention(C.Structure):
     _fields_ = [
         ("B", i32), ("T", i32), ("H", i32), ("dh", i32), ("dtype", i32), ("attn_scale", f32),
         ("q", vp), ("k", vp), ("v", vp), ("scores", vp), ("pattern", vp), ("z", vp),
+        ("causal", i32),
     ]
 
 
@@ -85,8 +86,23 @@ class PbVitForward(C.Structure):
     )
 
 
+class PbTextForward(C.Structure):
+    _fields_ = (
+        [(n, i32) for n in (
+            "batch", "n_tokens", "vocab", "d_model", "n_heads", "d_head", "d_mlp", "n_classes", "n_layers",
+            "causal", "normalize_output", "head_proj", "act", "dtype", "gemm_impl")]
+        + [("eps", f32), ("attn_scale", f32), ("ids", vp)]
+        + [(n, vp) for n in ("token_w", "pos", "lnf_w", "lnf_b", "head_w", "head_w_lo", "head_b")]
+        + [("layers_host", C.POINTER(PbVitLayerW)), ("embed", vp), ("full_embed", vp),
+           ("spills_host", C.POINTER(PbVitLayerSpill))]
+        + [(n, vp) for n in ("lnf_scale", "lnf_norm_f32", "lnf_out", "pooled", "pre_normalize", "out", "lo_scratch")]
+    )
+
+
 # index == argument of pb_abi_sizeof(); the layout test walks this list
 ABI_STRUCTS = [PbGemm, PbLayerNorm, PbAttention, PbVitLayerW, PbVitLayerSpill, PbVitForward]
+# indices past the SAE / peer-memory structs that sae_engine.py and p2p.py append (6-9)
+ABI_TEXT_FORWARD = 10
 
 # name -> (restype, argtypes); also the list the "exports every declared symbol" test walks
 SIGNATURES = {
@@ -111,7 +127,10 @@ SIGNATURES = {
     "pb_im2col_tubelets": (i32, [vp, vp, i32, i32, i32, i32, i32, i32, i32, vp]),
     "pb_embed_assemble": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, i32, vp]),
     "pb_cast": (i32, [vp, i32, vp, i32, i64, vp]),
+    "pb_embed_tokens": (i32, [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp]),
+    "pb_gather_argmax_rows": (i32, [vp, vp, vp, i32, i32, i32, i32, vp]),
     "pb_vit_forward": (i32, [C.POINTER(PbVitForward), vp]),
+    "pb_text_forward": (i32, [C.POINTER(PbTextForward), vp]),
 }
 
 _lib = None

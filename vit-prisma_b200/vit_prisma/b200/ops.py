@@ -203,10 +203,12 @@ def attn_pv(pattern: torch.Tensor, v: torch.Tensor) -> torch.Tensor:
     return z
 
 
-def attention(q, k, v, attn_scale: float, want_scores: bool = True, want_pattern: bool = True):
+def attention(q, k, v, attn_scale: float, want_scores: bool = True, want_pattern: bool = True, causal: bool = False):
+    """Fused scores -> softmax -> PV; ``causal`` scores key j > query i as -inf (the text towers' additive mask)."""
     _need_cuda(q, k, v)
     q, k, v = q.contiguous(), k.contiguous(), v.contiguous()
     p, (B, T, H, dh) = _att_desc(q, k, v, attn_scale)
+    p.causal = int(causal)
     scores = torch.empty((B, H, T, T), dtype=q.dtype, device=q.device) if want_scores else None
     pattern = torch.empty((B, H, T, T), dtype=q.dtype, device=q.device) if want_pattern else None
     z = torch.empty((B, T, H, dh), dtype=q.dtype, device=q.device)
@@ -287,6 +289,33 @@ def im2col_tubelets(videos: torch.Tensor, patch: int, depth: int) -> torch.Tenso
     out = torch.empty((B * nt * g * g, Cc * depth * patch * patch), dtype=videos.dtype, device=videos.device)
     L.check(L.get_lib().pb_im2col_tubelets(videos.data_ptr(), out.data_ptr(), B, Cc, F, S, patch, depth, dtype_code(videos.dtype),
                                            _stream()), "pb_im2col_tubelets")
+    return out
+
+
+def embed_tokens(ids: torch.Tensor, W_E: torch.Tensor, pos: torch.Tensor):
+    """ids int64 [B,T] -> (hook_embed = W_E[ids], full = embed + pos[:T]), both [B,T,d] in W_E's dtype.  Ids must lie in
+    [0, vocab): the kernel never reads outside W_E, and fills rows of out-of-range ids with NaN."""
+    _need_cuda(ids, W_E, pos)
+    assert ids.dtype == torch.int64 and ids.dim() == 2 and pos.dtype == W_E.dtype and pos.shape[0] >= ids.shape[1]
+    ids, W_E, pos = ids.contiguous(), W_E.contiguous(), pos.contiguous()
+    B, T = ids.shape
+    vocab, d = W_E.shape
+    embed = torch.empty((B, T, d), dtype=W_E.dtype, device=W_E.device)
+    full = torch.empty_like(embed)
+    L.check(L.get_lib().pb_embed_tokens(ids.data_ptr(), W_E.data_ptr(), pos.data_ptr(), embed.data_ptr(), full.data_ptr(), B, T, d,
+                                        vocab, dtype_code(W_E.dtype), _stream()), "pb_embed_tokens")
+    return embed, full
+
+
+def gather_argmax_rows(ids: torch.Tensor, x: torch.Tensor) -> torch.Tensor:
+    """``x[arange(B), ids.argmax(-1)]`` for ids int64 [B,T] and x [B,T,d] (first maximal index on ties)."""
+    _need_cuda(ids, x)
+    assert ids.dtype == torch.int64 and ids.shape == x.shape[:2]
+    ids, x = ids.contiguous(), x.contiguous()
+    B, T, d = x.shape
+    out = torch.empty((B, d), dtype=x.dtype, device=x.device)
+    L.check(L.get_lib().pb_gather_argmax_rows(ids.data_ptr(), x.data_ptr(), out.data_ptr(), B, T, d, dtype_code(x.dtype), _stream()),
+            "pb_gather_argmax_rows")
     return out
 
 

@@ -59,7 +59,136 @@ def _make_norm(cfg):
     raise ValueError(f"Invalid normalization type: {cfg.normalization_type}")
 
 
-class HookedViT(HookedRootModule):
+def init_he(model: nn.Module) -> None:
+    """The reference's ``weight_type == "he"`` initialisation of every submodule (base_vit.py, base_text_transformer.py)."""
+    cfg = model.cfg
+    for m in model.modules():
+        if isinstance(m, PosEmbedding):
+            nn.init.normal_(m.W_pos, std=cfg.pos_std)
+        elif isinstance(m, Attention):
+            for w in (m.W_Q, m.W_K, m.W_V, m.W_O):
+                nn.init.xavier_uniform_(w)
+        elif isinstance(m, MLP):
+            nn.init.kaiming_normal_(m.W_in, nonlinearity="relu")
+            nn.init.kaiming_normal_(m.W_out, nonlinearity="relu")
+            nn.init.zeros_(m.b_out)
+            nn.init.zeros_(m.b_in)
+        elif isinstance(m, Head):
+            nn.init.kaiming_normal_(m.W_H, nonlinearity="relu")
+            nn.init.zeros_(m.b_H)
+        elif isinstance(m, (nn.Linear, nn.Conv2d)):
+            nn.init.kaiming_normal_(m.weight, nonlinearity="relu")
+            if m.bias is not None:
+                nn.init.constant_(m.bias, 0)
+
+
+class _TwoRouteModel(HookedRootModule):
+    """Route choice, host staging, ``run_with_cache`` and device moves shared by the hooked towers.
+
+    A subclass provides ``_probe()`` (the parameter whose device and dtype stand for the model's), ``_fusable_reason(x)``
+    (None when its fused engine can serve ``x``) and ``self._engine`` (whose ``run(x, want, stop_at_layer)`` returns
+    ``(out, cache)``)."""
+
+    def _probe(self) -> torch.Tensor:
+        raise NotImplementedError
+
+    def _fusable_reason(self, x) -> Optional[str]:
+        raise NotImplementedError
+
+    # ------------------------------------------------------------ route choice
+    def _fused_blocker(self, x) -> Optional[str]:
+        """Why the fused chain cannot serve this call (None = it can)."""
+        if os.environ.get("PRISMA_B200_ROUTE") == "hooked":
+            return "forced by PRISMA_B200_ROUTE"
+        why = self._fusable_reason(x)
+        if why:
+            return why
+        if _global_module_hooks_present():
+            return "global torch module hooks registered"
+        for mod in self.modules():
+            if mod._forward_hooks or mod._forward_pre_hooks or mod._backward_hooks or mod._backward_pre_hooks:
+                return f"torch hook registered on {getattr(mod, 'name', type(mod).__name__)}"
+        return None
+
+    # ----------------------------------------------------------------- host-resident models
+    # Device policy: vit_prisma/b200/staging.py.  A model whose parameters live in host memory (the reference's default
+    # ``HookedViTConfig.device = "cpu"``) is staged on the GPU for the duration of a call; nothing ever computes on the CPU.
+    def _host_resident(self) -> bool:
+        return not self._probe().is_cuda
+
+    def _staged_on_gpu(self):
+        return staged_on_gpu(self)
+
+    @staticmethod
+    def _to_like(obj, device):
+        return _move(obj, device)
+
+    # ----------------------------------------------------------------- caching
+    def run_with_cache(self, *model_args, return_cache_object: bool = True, remove_batch_dim: bool = False, **kwargs
+                       ) -> Tuple[torch.Tensor, Union[ActivationCache, Dict[str, torch.Tensor]]]:
+        """``(model_out, cache)``; cache is an ActivationCache unless ``return_cache_object=False``.
+
+        Accepts every keyword of the reference (names_filter, device, incl_bwd, reset_hooks_end,
+        clear_contexts, fwd_hooks, bwd_hooks, stop_at_layer, ...).  The fused route is used when the
+        only thing attached to the model would have been the internal save-hook."""
+        out, cache_dict = self._run_with_cache_impl(*model_args, remove_batch_dim=remove_batch_dim, **kwargs)
+        if return_cache_object:
+            return out, ActivationCache(cache_dict, self, has_batch_dim=not remove_batch_dim)
+        return out, cache_dict
+
+    def _run_with_cache_impl(self, *model_args, names_filter=None, device=None, remove_batch_dim=False,
+                             incl_bwd=False, reset_hooks_end=True, clear_contexts=False, fwd_hooks=[],
+                             bwd_hooks=[], **model_kwargs):
+        if model_args and isinstance(model_args[0], torch.Tensor) and self._host_resident():
+            home = model_args[0].device                              # host-resident model: stage, run on the GPU, bring results home
+            with self._staged_on_gpu():
+                out, cache = self._run_with_cache_impl(model_args[0].to("cuda"), *model_args[1:], names_filter=names_filter,
+                                                       device=device if device is not None else home, remove_batch_dim=remove_batch_dim,
+                                                       incl_bwd=incl_bwd, reset_hooks_end=reset_hooks_end, clear_contexts=clear_contexts,
+                                                       fwd_hooks=fwd_hooks, bwd_hooks=bwd_hooks, **model_kwargs)
+            return self._to_like(out, home), cache
+        if model_args and isinstance(model_args[0], torch.Tensor) and not model_args[0].is_cuda:
+            model_args = (model_args[0].to(self._probe().device),) + tuple(model_args[1:])
+        plain = (len(model_args) == 1 and not incl_bwd and not fwd_hooks and not bwd_hooks
+                 and set(model_kwargs) <= {"stop_at_layer"})
+        why = self._fused_blocker(model_args[0]) if plain else "user hooks / backward requested"
+        if why is None:
+            self.last_route = "fused"
+            want = normalise_names_filter(names_filter)
+            known = self.hook_dict
+            out, cache = self._engine.run(model_args[0], lambda n: n in known and want(n), model_kwargs.get("stop_at_layer"))
+            if device is not None or remove_batch_dim:
+                for key, val in cache.items():
+                    val = val.to(device) if device is not None else val
+                    cache[key] = val[0] if remove_batch_dim else val
+            # mirror the reference's side effects of a caching run
+            self.is_caching = False
+            return out, cache
+        self.last_route = f"hooked: {why}"
+        return super().run_with_cache(*model_args, names_filter=names_filter, device=device,
+                                      remove_batch_dim=remove_batch_dim, incl_bwd=incl_bwd,
+                                      reset_hooks_end=reset_hooks_end, clear_contexts=clear_contexts,
+                                      fwd_hooks=fwd_hooks, bwd_hooks=bwd_hooks, **model_kwargs)
+
+    # ------------------------------------------------------- device / dtype moves
+    def to(self, *args, **kwargs):
+        """``nn.Module.to`` that also keeps ``cfg.device`` / ``cfg.dtype`` truthful -- the kernels pick
+        their arithmetic type from ``cfg.dtype`` (the reference's LayerNorm does the same, layer_norm.py:82)."""
+        out = super().to(*args, **kwargs)
+        probe = self._probe()
+        self.cfg.device = str(probe.device)
+        if probe.dtype != self.cfg.dtype and probe.dtype.is_floating_point:
+            self.cfg.dtype = probe.dtype
+        return out
+
+    def cuda(self, device=None):
+        return self.to("cuda" if device is None else device)
+
+    def cpu(self):
+        return self.to("cpu")
+
+
+class HookedViT(_TwoRouteModel):
     def __init__(self, cfg: Union[HookedViTConfig, Dict]):
         super().__init__()
         if isinstance(cfg, Dict):
@@ -96,33 +225,11 @@ class HookedViT(HookedRootModule):
         self._engine = VitEngine(self)
         self.last_route: Optional[str] = None   # "fused" | "hooked: <why>" -- introspection for tests/bench
 
-    # ------------------------------------------------------------ route choice
-    def _fused_blocker(self, x) -> Optional[str]:
-        """Why the fused chain cannot serve this call (None = it can)."""
-        if os.environ.get("PRISMA_B200_ROUTE") == "hooked":
-            return "forced by PRISMA_B200_ROUTE"
-        why = fusable_reason(self, x)
-        if why:
-            return why
-        if _global_module_hooks_present():
-            return "global torch module hooks registered"
-        for mod in self.modules():
-            if mod._forward_hooks or mod._forward_pre_hooks or mod._backward_hooks or mod._backward_pre_hooks:
-                return f"torch hook registered on {getattr(mod, 'name', type(mod).__name__)}"
-        return None
+    def _probe(self) -> torch.Tensor:
+        return self.cls_token
 
-    # ----------------------------------------------------------------- host-resident models
-    # Device policy: vit_prisma/b200/staging.py.  A model whose parameters live in host memory (the reference's default
-    # ``HookedViTConfig.device = "cpu"``) is staged on the GPU for the duration of a call; nothing ever computes on the CPU.
-    def _host_resident(self) -> bool:
-        return not self.cls_token.is_cuda
-
-    def _staged_on_gpu(self):
-        return staged_on_gpu(self)
-
-    @staticmethod
-    def _to_like(obj, device):
-        return _move(obj, device)
+    def _fusable_reason(self, x) -> Optional[str]:
+        return fusable_reason(self, x)
 
     # ----------------------------------------------------------------- forward
     def forward(self, input: torch.Tensor, stop_at_layer: Optional[int] = None):
@@ -173,95 +280,13 @@ class HookedViT(HookedRootModule):
             x = ops.l2_normalize_rows(x)
         return x
 
-    # ----------------------------------------------------------------- caching
-    def run_with_cache(self, *model_args, return_cache_object: bool = True, remove_batch_dim: bool = False, **kwargs
-                       ) -> Tuple[torch.Tensor, Union[ActivationCache, Dict[str, torch.Tensor]]]:
-        """``(model_out, cache)``; cache is an ActivationCache unless ``return_cache_object=False``.
-
-        Accepts every keyword of the reference (names_filter, device, incl_bwd, reset_hooks_end,
-        clear_contexts, fwd_hooks, bwd_hooks, stop_at_layer, ...).  The fused route is used when the
-        only thing attached to the model would have been the internal save-hook."""
-        out, cache_dict = self._run_with_cache_impl(*model_args, remove_batch_dim=remove_batch_dim, **kwargs)
-        if return_cache_object:
-            return out, ActivationCache(cache_dict, self, has_batch_dim=not remove_batch_dim)
-        return out, cache_dict
-
-    def _run_with_cache_impl(self, *model_args, names_filter=None, device=None, remove_batch_dim=False,
-                             incl_bwd=False, reset_hooks_end=True, clear_contexts=False, fwd_hooks=[],
-                             bwd_hooks=[], **model_kwargs):
-        if model_args and isinstance(model_args[0], torch.Tensor) and self._host_resident():
-            home = model_args[0].device                              # host-resident model: stage, run on the GPU, bring results home
-            with self._staged_on_gpu():
-                out, cache = self._run_with_cache_impl(model_args[0].to("cuda"), *model_args[1:], names_filter=names_filter,
-                                                       device=device if device is not None else home, remove_batch_dim=remove_batch_dim,
-                                                       incl_bwd=incl_bwd, reset_hooks_end=reset_hooks_end, clear_contexts=clear_contexts,
-                                                       fwd_hooks=fwd_hooks, bwd_hooks=bwd_hooks, **model_kwargs)
-            return self._to_like(out, home), cache
-        if model_args and isinstance(model_args[0], torch.Tensor) and not model_args[0].is_cuda:
-            model_args = (model_args[0].to(self.cls_token.device),) + tuple(model_args[1:])
-        plain = (len(model_args) == 1 and not incl_bwd and not fwd_hooks and not bwd_hooks
-                 and set(model_kwargs) <= {"stop_at_layer"})
-        why = self._fused_blocker(model_args[0]) if plain else "user hooks / backward requested"
-        if why is None:
-            self.last_route = "fused"
-            want = normalise_names_filter(names_filter)
-            known = self.hook_dict
-            out, cache = self._engine.run(model_args[0], lambda n: n in known and want(n), model_kwargs.get("stop_at_layer"))
-            if device is not None or remove_batch_dim:
-                for key, val in cache.items():
-                    val = val.to(device) if device is not None else val
-                    cache[key] = val[0] if remove_batch_dim else val
-            # mirror the reference's side effects of a caching run
-            self.is_caching = False
-            return out, cache
-        self.last_route = f"hooked: {why}"
-        return super().run_with_cache(*model_args, names_filter=names_filter, device=device,
-                                      remove_batch_dim=remove_batch_dim, incl_bwd=incl_bwd,
-                                      reset_hooks_end=reset_hooks_end, clear_contexts=clear_contexts,
-                                      fwd_hooks=fwd_hooks, bwd_hooks=bwd_hooks, **model_kwargs)
-
     # -------------------------------------------------------------------- init
     def init_weights(self) -> None:
         cfg = self.cfg
         if cfg.use_cls_token:
             nn.init.normal_(self.cls_token, std=cfg.cls_std)
-        if cfg.weight_type != "he":
-            return
-        for m in self.modules():
-            if isinstance(m, PosEmbedding):
-                nn.init.normal_(m.W_pos, std=cfg.pos_std)
-            elif isinstance(m, Attention):
-                for w in (m.W_Q, m.W_K, m.W_V, m.W_O):
-                    nn.init.xavier_uniform_(w)
-            elif isinstance(m, MLP):
-                nn.init.kaiming_normal_(m.W_in, nonlinearity="relu")
-                nn.init.kaiming_normal_(m.W_out, nonlinearity="relu")
-                nn.init.zeros_(m.b_out)
-                nn.init.zeros_(m.b_in)
-            elif isinstance(m, Head):
-                nn.init.kaiming_normal_(m.W_H, nonlinearity="relu")
-                nn.init.zeros_(m.b_H)
-            elif isinstance(m, (nn.Linear, nn.Conv2d)):
-                nn.init.kaiming_normal_(m.weight, nonlinearity="relu")
-                if m.bias is not None:
-                    nn.init.constant_(m.bias, 0)
-
-    # ------------------------------------------------------- device / dtype moves
-    def to(self, *args, **kwargs):
-        """``nn.Module.to`` that also keeps ``cfg.device`` / ``cfg.dtype`` truthful -- the kernels pick
-        their arithmetic type from ``cfg.dtype`` (the reference's LayerNorm does the same, layer_norm.py:82)."""
-        out = super().to(*args, **kwargs)
-        probe = self.cls_token
-        self.cfg.device = str(probe.device)
-        if probe.dtype != self.cfg.dtype and probe.dtype.is_floating_point:
-            self.cfg.dtype = probe.dtype
-        return out
-
-    def cuda(self, device=None):
-        return self.to("cuda" if device is None else device)
-
-    def cpu(self):
-        return self.to("cpu")
+        if cfg.weight_type == "he":
+            init_he(self)
 
     # --------------------------------------------------------- toggles / checks
     def set_use_attn_result(self, use_attn_result: bool):

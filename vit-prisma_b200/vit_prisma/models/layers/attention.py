@@ -102,7 +102,10 @@ class Attention(nn.Module):
     def calculate_attn_scores(self, q, k, attention_mask=None):
         scores = ops.attn_scores(q, k, float(self.attn_scale))
         if attention_mask is not None:
-            scores = ops.add(scores, attention_mask.to(scores.dtype).unsqueeze(1).expand_as(scores))
+            mask = attention_mask.to(scores.dtype)
+            # [T, T] (the text towers' causal mask) broadcasts over batch and head as in the reference's
+            # ``scores + mask``; [B, T, T] gets a head axis
+            scores = ops.add(scores, (mask if mask.dim() == 2 else mask.unsqueeze(1)).expand_as(scores))
         return scores
 
     def calculate_z_scores(self, v, pattern):
