@@ -134,9 +134,19 @@ def test_layernorm(rows, cols, dtype):
 
 
 # -------------------------------------------------------------- attention
-@pytest.mark.parametrize("B,T,H,dh", [(2, 5, 4, 8), (3, 50, 12, 64), (1, 197, 2, 64), (1, 257, 2, 64), (2, 17, 2, 24)])
+def _offset_by_one(t):
+    """The same values in a contiguous view one element into its storage: not 16-byte aligned."""
+    buf = torch.empty(t.numel() + 1, dtype=t.dtype, device=t.device)
+    buf[1:] = t.reshape(-1)
+    return buf[1:].view(t.shape)
+
+
+# d_head 64: T <= 128 whole-row tensor-core kernel, T > 128 the 64-key-chunk one; unaligned q/k/v and other d_head: FFMA kernel
+@pytest.mark.parametrize("B,T,H,dh,unaligned", [(2, 5, 4, 8, False), (3, 50, 12, 64, False), (1, 197, 2, 64, False), (1, 257, 2, 64, False),
+                                                (2, 17, 2, 24, False), (2, 64, 3, 64, False), (2, 65, 3, 64, False), (2, 128, 3, 64, False),
+                                                (2, 129, 3, 64, False), (2, 50, 3, 64, True)])
 @pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16])
-def test_attention_fused_and_split(B, T, H, dh, dtype):
+def test_attention_fused_and_split(B, T, H, dh, unaligned, dtype):
     ops = _ops()
     q, k, v = (_rand(B, T, H, dh, seed=s, dtype=dtype) for s in (1, 2, 3))
     scale = math.sqrt(dh)
@@ -144,17 +154,24 @@ def test_attention_fused_and_split(B, T, H, dh, dtype):
     pt_ref = F.softmax(sc_ref.float(), dim=-1).to(dtype)
     z_ref = torch.einsum("bkhe,bhqk->bqhe", v.float(), pt_ref.float()).to(dtype)
     tol = 1e-5 if dtype == torch.float32 else 1.2e-2   # fp32: 3xTF32 products (d_head 64) / FFMA, fp32 accumulation
-    sc, pt, z = ops.attention(q.cuda(), k.cuda(), v.cuda(), scale)
+    if unaligned:
+        q, k, v = (_offset_by_one(x.cuda()) for x in (q, k, v))
+        assert all(x.data_ptr() % 16 for x in (q, k, v))
+    else:
+        q, k, v = q.cuda(), k.cuda(), v.cuda()
+    sc, pt, z = ops.attention(q, k, v, scale)
     assert rel_err(sc.float(), sc_ref.float()) < tol
     assert rel_err(pt.float(), pt_ref.float()) < tol
     assert rel_err(z.float(), z_ref.float()) < tol
     # not materialising scores / pattern must not change z
-    _, _, z2 = ops.attention(q.cuda(), k.cuda(), v.cuda(), scale, want_scores=False, want_pattern=False)
+    _, _, z2 = ops.attention(q, k, v, scale, want_scores=False, want_pattern=False)
     assert torch.equal(z2, z)
     # split route used by the hooked path
-    sc3 = ops.attn_scores(q.cuda(), k.cuda(), scale)
+    sc3 = ops.attn_scores(q, k, scale)
     pt3 = ops.softmax_rows(sc3)
-    z3 = ops.attn_pv(pt3, v.cuda())
+    z3 = ops.attn_pv(pt3, v)
+    if unaligned or dh != 64:   # the fused call took the FFMA kernel too: the same scores bit for bit
+        assert torch.equal(sc3, sc)
     # (d_head == 64 runs the mma.sync kernel when fused and the FFMA kernel when split: close, not bit-equal)
     assert rel_err(sc3.float(), sc.float()) < tol
     assert rel_err(pt3.float(), pt.float()) < tol and rel_err(z3.float(), z.float()) < tol

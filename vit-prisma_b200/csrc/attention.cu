@@ -16,11 +16,15 @@
 // Arithmetic is fp32; in bf16 mode values are rounded to bf16 exactly where the reference
 // materialises a bf16 tensor (scores, pattern, z).
 #include "common.cuh"
-#include <stdlib.h>
 
-int pb_attention_mma(const PbAttention* p, cudaStream_t st);  // attention_mma.cu
-int pb_attn_scores_long(const PbAttention* p, cudaStream_t st);  // attention_long.cu
+// the d_head == 64 tensor-core kernels; callers guarantee d_head == 64 and 16-byte aligned operands
+int pb_attention_mma(const PbAttention* p, cudaStream_t st);     // attention_mma.cu: T <= 128
+int pb_attention_long(const PbAttention* p, cudaStream_t st);    // attention_long.cu: any T
+int pb_attn_scores_long(const PbAttention* p, cudaStream_t st);
 int pb_attn_pv_long(const PbAttention* p, cudaStream_t st);
+
+// every pointer 16-byte aligned: the tensor-core kernels move head rows in 16-byte vectors
+template <typename... P> static bool aligned16(const P*... p) { return !((reinterpret_cast<uintptr_t>(p) | ...) & 15); }
 
 enum { ATT_FUSED = 0, ATT_SCORES = 1, ATT_PV = 2 };
 
@@ -232,30 +236,26 @@ static int check_att(const PbAttention* p, const char* who) {
 // Beyond the 608 tokens of the FFMA kernel the split stages run the tensor-core modes of attention_long.cu, which exist for
 // d_head == 64 only.  Up to 608 tokens the FFMA kernel keeps serving them, so shorter sequences keep their results.
 constexpr int ATT_SIMT_MAX_T = 608;
-static int split_long(int (*fn)(const PbAttention*, cudaStream_t), const PbAttention* p, cudaStream_t st, const char* who) {
+static int split_long(int (*fn)(const PbAttention*, cudaStream_t), const PbAttention* p, cudaStream_t st, const char* who, bool aligned) {
   if (p->dh != 64) {
     pb_set_error("%s: T=%d with d_head=%d unsupported: beyond %d tokens only d_head 64 is supported", who, p->T, p->dh, ATT_SIMT_MAX_T);
     return PB_EUNSUPPORTED;
   }
-  const int rc = fn(p, st);
-  if (rc == PB_EUNSUPPORTED) pb_set_error("%s: T=%d d_head=%d needs 16-byte aligned q/k/v/z pointers", who, p->T, p->dh);
-  return rc;
+  if (!aligned) {
+    pb_set_error("%s: T=%d d_head=%d needs 16-byte aligned q/k/v/z pointers", who, p->T, p->dh);
+    return PB_EUNSUPPORTED;
+  }
+  return fn(p, st);
 }
 
 extern "C" int pb_attention(const PbAttention* p, pb_stream_t stream) {
   PB_TRY(check_att(p, "pb_attention"));
   PB_CHECK_ARG(p->q && p->k && p->v && p->z, "pb_attention: q, k, v, z are required");
   if (p->B == 0) return PB_OK;
-  {
-    // d_head == 64, T <= 272: tensor-core kernel (attention_mma.cu); PB_ATTN_IMPL=simt forces the FFMA kernel (cross-check)
-    static int force_simt = -1;
-    if (force_simt < 0) { const char* e = getenv("PB_ATTN_IMPL"); force_simt = (e && !strcmp(e, "simt")) ? 1 : 0; }
-    if (!force_simt) {
-      const int rc = pb_attention_mma(p, (cudaStream_t)stream);
-      if (rc != PB_EUNSUPPORTED) return rc;
-    }
-  }
   cudaStream_t st = (cudaStream_t)stream;
+  // d_head == 64 with 16-byte aligned q / k / v / z: tensor cores, whole rows up to 128 tokens, 64-key chunks beyond;
+  // anything else: the FFMA kernel
+  if (p->dh == 64 && aligned16(p->q, p->k, p->v, p->z)) return p->T <= 128 ? pb_attention_mma(p, st) : pb_attention_long(p, st);
   if (p->causal) return p->dtype == PB_F32 ? launch_att<float, ATT_FUSED, true>(p, st) : launch_att<bf16, ATT_FUSED, true>(p, st);
   return p->dtype == PB_F32 ? launch_att<float, ATT_FUSED>(p, st) : launch_att<bf16, ATT_FUSED>(p, st);
 }
@@ -263,14 +263,14 @@ extern "C" int pb_attn_scores(const PbAttention* p, pb_stream_t stream) {
   PB_TRY(check_att(p, "pb_attn_scores"));
   PB_CHECK_ARG(p->q && p->k && p->scores, "pb_attn_scores: q, k, scores are required");
   if (p->B == 0) return PB_OK;
-  if (p->T > ATT_SIMT_MAX_T) return split_long(pb_attn_scores_long, p, (cudaStream_t)stream, "pb_attn_scores");
+  if (p->T > ATT_SIMT_MAX_T) return split_long(pb_attn_scores_long, p, (cudaStream_t)stream, "pb_attn_scores", aligned16(p->q, p->k));
   return p->dtype == PB_F32 ? launch_att<float, ATT_SCORES>(p, (cudaStream_t)stream) : launch_att<bf16, ATT_SCORES>(p, (cudaStream_t)stream);
 }
 extern "C" int pb_attn_pv(const PbAttention* p, pb_stream_t stream) {
   PB_TRY(check_att(p, "pb_attn_pv"));
   PB_CHECK_ARG(p->pattern && p->v && p->z, "pb_attn_pv: pattern, v, z are required");
   if (p->B == 0) return PB_OK;
-  if (p->T > ATT_SIMT_MAX_T) return split_long(pb_attn_pv_long, p, (cudaStream_t)stream, "pb_attn_pv");
+  if (p->T > ATT_SIMT_MAX_T) return split_long(pb_attn_pv_long, p, (cudaStream_t)stream, "pb_attn_pv", aligned16(p->v, p->z));
   return p->dtype == PB_F32 ? launch_att<float, ATT_PV>(p, (cudaStream_t)stream) : launch_att<bf16, ATT_PV>(p, (cudaStream_t)stream);
 }
 

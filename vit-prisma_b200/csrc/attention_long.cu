@@ -20,53 +20,12 @@
 // slab is one 64-row chunk, so key chunks past the slab lie wholly above the diagonal: neither pass loads or multiplies them,
 // and a requested spill gets -inf / 0 there.  Every processed chunk has key kc0 <= each row of the slab, so the running max of
 // a row is finite from chunk 0 on; masked entries are still kept out of the running sum explicitly.
-#include "common.cuh"
+#include "attention_frag.cuh"
 
 namespace {
 
-__device__ __forceinline__ void mma_bf16(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], const uint32_t (&b)[2]) {
-  asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
-}
-// 3xTF32 with the A operand already split (Q fragments live in registers across all chunks)
-__device__ __forceinline__ void mma_tf32x3_presplit(float (&d)[4], const uint32_t (&ah)[4], const uint32_t (&al)[4], const float (&b)[2]) {
-  uint32_t bh[2], bl[2];
-#pragma unroll
-  for (int i = 0; i < 2; ++i) { bh[i] = __float_as_uint(b[i]); bl[i] = __float_as_uint(tf32_lo(b[i])); }
-  mma_tf32(d, al, bh);
-  mma_tf32(d, ah, bl);
-  mma_tf32(d, ah, bh);
-}
-__device__ __forceinline__ void mma_tf32x3(float (&d)[4], const float (&a)[4], const float (&b)[2]) {
-  uint32_t ah[4], al[4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) { ah[i] = __float_as_uint(a[i]); al[i] = __float_as_uint(tf32_lo(a[i])); }
-  mma_tf32x3_presplit(d, ah, al, b);
-}
-__device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
-  __nv_bfloat162 t = __floats2bfloat162_rn(lo, hi);
-  return *reinterpret_cast<uint32_t*>(&t);
-}
-__device__ __forceinline__ void ldmatrix_x4(uint32_t (&r)[4], const void* smem_row) {
-  const uint32_t a = (uint32_t)__cvta_generic_to_shared(smem_row);
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(a));
-}
-__device__ __forceinline__ void ldmatrix_x4_trans(uint32_t (&r)[4], const void* smem_row) {
-  const uint32_t a = (uint32_t)__cvta_generic_to_shared(smem_row);
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(a));
-}
-
-constexpr int DH = 64;
 constexpr int KC = 64;                                    // keys per chunk
 enum { LONG_FUSED = 0, LONG_SCORES = 1, LONG_PV = 2 };
-template <typename T> struct Lay { static constexpr int LD = DH + (sizeof(T) == 2 ? 8 : 4); };
-
 __device__ __forceinline__ void stage_put(float* p, float a, float b) { p[0] = a; p[1] = b; }
 __device__ __forceinline__ void stage_put(bf16* p, float a, float b) { *reinterpret_cast<uint32_t*>(p) = pack_bf16(a, b); }
 
@@ -383,41 +342,27 @@ template <typename T, int MODE, bool CAUSAL = false>
 int launch_long(const PbAttention* p, cudaStream_t st) {
   constexpr int NW = 4;
   const size_t smem = ((size_t)(NW * 16 + 2 * KC) * Lay<T>::LD + (size_t)NW * 16 * KC) * sizeof(T);
-  auto kern = k_attention_long<T, NW, MODE, CAUSAL>;
-  static bool attr_done = false;
-  if (!attr_done && smem > 48 * 1024) {
-    PB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_done = true;
-  }
-  int ex = 0;
-  const float mant = frexpf(p->attn_scale, &ex);
-  const float inv_scale = (mant == 0.5f) ? 1.f / p->attn_scale : 0.f;
+  constexpr auto kern = k_attention_long<T, NW, MODE, CAUSAL>;
+  PB_TRY(smem_opt_in<kern>(smem));
   dim3 grid(p->B * p->H, (p->T + NW * 16 - 1) / (NW * 16));
   kern<<<grid, NW * 32, smem, st>>>((const T*)p->q, (const T*)p->k, (const T*)p->v, (T*)p->scores, (T*)p->pattern, (T*)p->z, p->T, p->H,
-                                    p->attn_scale, inv_scale);
+                                    p->attn_scale, pow2_inv_scale(p->attn_scale));
   PB_LAUNCH_CHECK();
   return PB_OK;
 }
 
 }  // namespace
 
-// d_head == 64, any T (used for T > 128); PB_EUNSUPPORTED when the pointers are not 16-byte aligned.
+// d_head == 64 and 16-byte aligned q / k / v / z, any T: pb_attention (attention.cu) routes T > 128 here.
 int pb_attention_long(const PbAttention* p, cudaStream_t st) {
-  if (p->dh != DH) return PB_EUNSUPPORTED;
-  if (((uintptr_t)p->q | (uintptr_t)p->k | (uintptr_t)p->v | (uintptr_t)p->z) & 15) return PB_EUNSUPPORTED;
   if (p->causal) return p->dtype == PB_F32 ? launch_long<float, LONG_FUSED, true>(p, st) : launch_long<bf16, LONG_FUSED, true>(p, st);
   return p->dtype == PB_F32 ? launch_long<float, LONG_FUSED>(p, st) : launch_long<bf16, LONG_FUSED>(p, st);
 }
 
-// The split stages for d_head == 64 (attention.cu routes T > 608 here): q, k -> scores and pattern, v -> z.
-// PB_EUNSUPPORTED when d_head != 64 or the q / k (scores) or v / z (pv) pointers are not 16-byte aligned.
+// The split stages for d_head == 64 with 16-byte aligned q / k (scores) or v / z (pv); attention.cu routes T > 608 here.
 int pb_attn_scores_long(const PbAttention* p, cudaStream_t st) {
-  if (p->dh != DH) return PB_EUNSUPPORTED;
-  if (((uintptr_t)p->q | (uintptr_t)p->k) & 15) return PB_EUNSUPPORTED;
   return p->dtype == PB_F32 ? launch_long<float, LONG_SCORES>(p, st) : launch_long<bf16, LONG_SCORES>(p, st);
 }
 int pb_attn_pv_long(const PbAttention* p, cudaStream_t st) {
-  if (p->dh != DH) return PB_EUNSUPPORTED;
-  if (((uintptr_t)p->v | (uintptr_t)p->z) & 15) return PB_EUNSUPPORTED;
   return p->dtype == PB_F32 ? launch_long<float, LONG_PV>(p, st) : launch_long<bf16, LONG_PV>(p, st);
 }

@@ -5,68 +5,13 @@
 // round trip would be mostly padding.  Warp-level mma.sync keeps S and P in registers between QK^T, softmax and PV.
 //
 // One CTA = one (batch, head) x one slab of NW*16 query rows; K, V (and the Q slab) of the head sit in shared memory,
-// row-major, copied in with 16-byte vectors (no conversion, no transposition on the way in).
-//   bf16 : mma.sync.m16n8k16 bf16 (fp32 accumulate); fragments come from ldmatrix (.trans for V, so the PV operand
-//          needs no transposed copy of V -- the transposing 2-byte stores of a first version were bank-conflict bound).
-//   fp32 : mma.sync.m16n8k8 tf32 in 3 passes (x = hi + lo, hi = what the tensor core reads of x, lo = x - hi:
-//          lo*hi + hi*lo + hi*hi) -> fp32-grade products for the 1e-4 parity bar.
-// Hook points leave through a per-warp stage that holds the warp's 16 rows packed exactly as they lie in global memory
-// ([16][T] elements of T, already rounded), so the copy-out is a linear vector memcpy of one contiguous run.
-// Rounding points follow the reference graph: scores = round(round(q.k) / scale); pattern = round(softmax);
-// z = round(pattern @ v) with the rounded pattern as the operand.
-#include <stdlib.h>
-
-#include "common.cuh"
-
-int pb_attention_long(const PbAttention* p, cudaStream_t st);   // attention_long.cu
+// row-major, copied in with 16-byte vectors (no conversion, no transposition on the way in); the mma.sync wrappers, operand
+// layouts and rounding points are those of attention_frag.cuh.  Hook points leave through a per-warp stage that holds the
+// warp's 16 rows packed exactly as they lie in global memory ([16][T] elements of T, already rounded), so the copy-out is a
+// linear vector memcpy of one contiguous run.
+#include "attention_frag.cuh"
 
 namespace {
-
-__device__ __forceinline__ void mma_bf16(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], const uint32_t (&b)[2]) {
-  asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
-}
-// 3xTF32: operands given as fp32 values
-__device__ __forceinline__ void mma_tf32x3(float (&d)[4], const float (&a)[4], const float (&b)[2]) {
-  uint32_t ah[4], al[4], bh[2], bl[2];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    ah[i] = __float_as_uint(a[i]);            // mma.sync reads the tf32 part of the word
-    al[i] = __float_as_uint(tf32_lo(a[i]));
-  }
-#pragma unroll
-  for (int i = 0; i < 2; ++i) {
-    bh[i] = __float_as_uint(b[i]);
-    bl[i] = __float_as_uint(tf32_lo(b[i]));
-  }
-  mma_tf32(d, al, bh);
-  mma_tf32(d, ah, bl);
-  mma_tf32(d, ah, bh);
-}
-__device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
-  __nv_bfloat162 t = __floats2bfloat162_rn(lo, hi);
-  return *reinterpret_cast<uint32_t*>(&t);
-}
-__device__ __forceinline__ void ldmatrix_x4(uint32_t (&r)[4], const void* smem_row) {
-  const uint32_t a = (uint32_t)__cvta_generic_to_shared(smem_row);
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(a));
-}
-__device__ __forceinline__ void ldmatrix_x4_trans(uint32_t (&r)[4], const void* smem_row) {
-  const uint32_t a = (uint32_t)__cvta_generic_to_shared(smem_row);
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(a));
-}
-
-constexpr int DH = 64;
-
-// shared-memory row stride of Q / K / V in elements: 144 B (bf16) / 272 B (fp32) -- 16-byte aligned rows whose 16 B
-// pieces rotate through the banks (ldmatrix, 128-bit copies and the scalar tf32 fragment loads are all conflict-free)
-template <typename T> struct Lay { static constexpr int LD = DH + (sizeof(T) == 2 ? 8 : 4); };
 
 // two adjacent columns (c even) of one stage row; only columns < Tn exist in the packed layout
 template <typename T> __device__ __forceinline__ void stage_put2(T* stage, int r, int c, int Tn, float a, float b);
@@ -330,55 +275,36 @@ int pow2_align(uint64_t x) {   // largest power of two <= 16 dividing x
   return a;
 }
 
-template <typename T, int NT, int NW, bool CAUSAL>
+template <typename T, int NT, bool CAUSAL>
 int launch_mma(const PbAttention* p, cudaStream_t st) {
-  constexpr int TPAD = NT * 8;
-  const size_t es = sizeof(T);
-  const size_t smem = ((size_t)2 * TPAD * Lay<T>::LD + (size_t)NW * 16 * Lay<T>::LD + (size_t)NW * 16 * TPAD) * es;
-  if (smem > 227 * 1024) return PB_EUNSUPPORTED;
-  auto kern = k_attention_mma<T, NT, NW, CAUSAL>;
-  static bool attr_done = false;
-  if (!attr_done && smem > 48 * 1024) {
-    PB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_done = true;
-  }
+  constexpr int NW = 4, TPAD = NT * 8;
+  constexpr size_t es = sizeof(T);
+  constexpr size_t smem = ((size_t)2 * TPAD * Lay<T>::LD + (size_t)NW * 16 * Lay<T>::LD + (size_t)NW * 16 * TPAD) * es;
+  static_assert(smem <= 227 * 1024, "K, V, the Q slab and the stages must fit in shared memory");
+  constexpr auto kern = k_attention_mma<T, NT, NW, CAUSAL>;
+  PB_TRY(smem_opt_in<kern>(smem));
   // vector width of the score / pattern copy-out: every warp run starts at base + ((bh*T + 16*w) * T) elements
   int vb = pow2_align((uint64_t)p->T * p->T * es);
   vb = min(vb, pow2_align((uint64_t)16 * p->T * es));
   if (p->scores) vb = min(vb, pow2_align((uint64_t)(uintptr_t)p->scores));
   if (p->pattern) vb = min(vb, pow2_align((uint64_t)(uintptr_t)p->pattern));
   if (vb < 4) vb = 0;
-  int ex = 0;
-  const float mant = frexpf(p->attn_scale, &ex);
-  const float inv_scale = (mant == 0.5f) ? 1.f / p->attn_scale : 0.f;
   dim3 grid(p->B * p->H, (p->T + NW * 16 - 1) / (NW * 16));
   kern<<<grid, NW * 32, smem, st>>>((const T*)p->q, (const T*)p->k, (const T*)p->v, (T*)p->scores, (T*)p->pattern, (T*)p->z, p->T, p->H,
-                                    p->attn_scale, inv_scale, vb);
+                                    p->attn_scale, pow2_inv_scale(p->attn_scale), vb);
   PB_LAUNCH_CHECK();
   return PB_OK;
 }
 
 template <typename T, bool CAUSAL>
 int dispatch_mma(const PbAttention* p, cudaStream_t st) {
-  if (p->T <= 64) return launch_mma<T, 8, 4, CAUSAL>(p, st);
-  if (p->T <= 128) return launch_mma<T, 16, 4, CAUSAL>(p, st);
-  // longer rows: K / V streamed in 64-key chunks, two passes (attention_long.cu); PB_ATTN_LONG=0 keeps the whole-row kernels
-  // below for cross-checks (T <= 272)
-  static int use_long = -1;
-  if (use_long < 0) { const char* e = getenv("PB_ATTN_LONG"); use_long = (e && !strcmp(e, "0")) ? 0 : 1; }
-  if (use_long) return pb_attention_long(p, st);
-  if (p->T <= 208) return launch_mma<T, 26, 2, CAUSAL>(p, st);
-  if (p->T <= 272) return launch_mma<T, 34, 2, CAUSAL>(p, st);
-  return PB_EUNSUPPORTED;
+  return p->T <= 64 ? launch_mma<T, 8, CAUSAL>(p, st) : launch_mma<T, 16, CAUSAL>(p, st);
 }
 
 }  // namespace
 
-// PB_OK when the tensor-core kernel took the call, PB_EUNSUPPORTED when the shape is not covered (caller falls back to
-// the FFMA kernel in attention.cu), anything else is an error.
+// d_head == 64, T <= 128, q / k / v / z 16-byte aligned: pb_attention (attention.cu) routes only such calls here
 int pb_attention_mma(const PbAttention* p, cudaStream_t st) {
-  if (p->dh != DH) return PB_EUNSUPPORTED;
-  if (((uintptr_t)p->q | (uintptr_t)p->k | (uintptr_t)p->v | (uintptr_t)p->z) & 15) return PB_EUNSUPPORTED;
   if (p->causal) return p->dtype == PB_F32 ? dispatch_mma<float, true>(p, st) : dispatch_mma<bf16, true>(p, st);
   return p->dtype == PB_F32 ? dispatch_mma<float, false>(p, st) : dispatch_mma<bf16, false>(p, st);
 }
