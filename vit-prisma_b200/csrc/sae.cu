@@ -330,7 +330,7 @@ __global__ void __launch_bounds__(256) k_sae_decode(const float* __restrict__ x,
     float a = 0.f, b = 0.f;
     for (int i = 0; i < (int)(blockDim.x >> 5); ++i) { a += red[0][i]; b += red[1][i]; }
     atomicAdd(&sc->loss_sum, a);
-    atomicAdd(&sc->pos_count, b);
+    atomicAdd(&sc->pos_count, (unsigned)b);                    // b: a whole count below 2^24, exact in fp32
   }
 }
 
@@ -1042,7 +1042,7 @@ extern "C" int pb_sae_scatter_acts(const int32_t* idx, const float* val, float* 
 // PbSaeStep: every pointer of one training / inference step (device memory owned by the caller)
 __global__ void k_sae_fwd_scalars(SaeScalars* sc, float inv_elems, float inv_rows) {
   sc->mse = sc->loss_sum * inv_elems;
-  sc->l0 = sc->pos_count * inv_rows;
+  sc->l0 = (float)sc->pos_count * inv_rows;
 }
 
 // every accumulator a training step starts from zero, in one launch (they were six memsets / fills on the stream)

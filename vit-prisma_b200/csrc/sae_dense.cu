@@ -79,7 +79,7 @@ __global__ void __launch_bounds__(256) k_dense_stats(const float* __restrict__ a
   if (threadIdx.x == 0) {
     float a = 0.f, b = 0.f;
     for (int i = 0; i < 8; ++i) { a += red[0][i]; b += red[1][i]; }
-    if (a != 0.f) atomicAdd(&sc->pos_count, a);
+    if (a != 0.f) atomicAdd(&sc->pos_count, (unsigned)a);     // a: a whole count below 2^24, exact in fp32
     if (b != 0.f) atomicAdd(l1_sum, b);
   }
 }
@@ -403,7 +403,7 @@ __global__ void __launch_bounds__(256) k_gated_fwd(const float* __restrict__ pi,
   if (threadIdx.x == 0) {
     float a = 0.f;
     for (int i = 0; i < 8; ++i) a += red[i];
-    if (a != 0.f) atomicAdd(&sc->pos_count, a);
+    if (a != 0.f) atomicAdd(&sc->pos_count, (unsigned)a);     // a: a whole count below 2^24, exact in fp32
   }
 }
 

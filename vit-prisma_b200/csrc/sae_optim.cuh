@@ -16,7 +16,7 @@ struct SaeScalars {
   float clip_coef;     // min(1, max_norm / (norm + 1e-6))
   float mse;           // loss_sum / (Bt*d)
   float l0;            // mean number of positive activations per token
-  float pos_count;     // accumulator for l0
+  unsigned pos_count;  // accumulator for l0: an integer, since an fp32 sum stops being exact past 2^24 positives
   float grad_norm;     // sqrt(gnorm_sq)
   float reserved;
 };
@@ -35,7 +35,7 @@ __device__ __forceinline__ void sae_publish_scalars(SaeScalars* sc, float gnorm_
   sc->grad_norm = norm;
   sc->clip_coef = sae_clip_coef(norm, max_norm);
   sc->mse = sc->loss_sum * inv_elems;
-  sc->l0 = sc->pos_count * inv_rows;
+  sc->l0 = (float)sc->pos_count * inv_rows;
 }
 
 // ---------------------------------------------------------------------------------------------

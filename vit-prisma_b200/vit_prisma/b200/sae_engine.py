@@ -442,6 +442,7 @@ class SaeStepEngine:
     def scalars_dict(self) -> dict:
         """Host read (synchronises): for logging / tests only."""
         vals = self.scalars.tolist()
+        vals[SCALAR_NAMES.index("pos_count")] = int(self.scalars.view(torch.int32)[SCALAR_NAMES.index("pos_count")])   # an integer slot
         return dict(zip(SCALAR_NAMES, vals))
 
     # algorithmic HBM bytes of one training step (SURVEY section 8d): 80*d*F + 8*Bt*d
