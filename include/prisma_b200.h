@@ -378,9 +378,6 @@ PB_API int pb_sae_dense_loss(const float* x, const float* out_n, const float* mu
                              pb_stream_t stream);
 /* d_hidden = (d_acts + l1_grad) * [acts > 0] in place on d_acts (+ optional tf32 residual): ReLU backward with d(l1)/d(acts) */
 PB_API int pb_sae_dense_dhid(float* d_acts, const float* acts, float* lo, float l1_grad, int64_t n, pb_stream_t stream);
-/* scalars: gnorm_sq = ||all four gradients||^2, grad_norm, clip_coef (train_sae.py:394-397), mse, l0 -- then pb_sae_adam */
-PB_API int pb_sae_grad_finish(const float* gW_dec, const float* gW_encT, const float* gb_enc, const float* gb_dec, int32_t F, int32_t d,
-                              void* scalars, float max_grad_norm, int32_t rows, pb_stream_t stream);
 /* E[r][j] = exp(hidden_pre[r][dead_idx[j]]), zero for nd <= j < ldE                                   (sae.py:164)  */
 PB_API int pb_sae_ghost_gather(const float* hidden_pre, const int32_t* dead_idx, int32_t nd, int32_t rows, int32_t F, float* E, int32_t ldE,
                                pb_stream_t stream);

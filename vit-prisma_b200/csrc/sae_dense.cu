@@ -299,26 +299,6 @@ extern "C" int pb_sae_dense_dhid(float* d_acts, const float* acts, float* lo, fl
   return PB_OK;
 }
 
-extern "C" int pb_sae_grad_finish(const float* gW_dec, const float* gW_encT, const float* gb_enc, const float* gb_dec, int32_t F, int32_t d,
-                                  void* scalars, float max_grad_norm, int32_t rows, pb_stream_t stream) {
-  PB_CHECK_ARG(gW_dec && gW_encT && gb_enc && gb_dec && scalars && F > 0 && d > 0 && rows > 0, "pb_sae_grad_finish: bad arguments");
-  cudaStream_t st = (cudaStream_t)stream;
-  SaeScalars* sc = (SaeScalars*)scalars;
-  PB_CUDA(cudaMemsetAsync(&sc->gnorm_sq, 0, sizeof(float), st));
-  const int64_t n = (int64_t)F * d;
-  k_sumsq<<<stream_grid(n), 256, 0, st>>>(gW_dec, n, &sc->gnorm_sq);
-  PB_LAUNCH_CHECK();
-  k_sumsq<<<stream_grid(n), 256, 0, st>>>(gW_encT, n, &sc->gnorm_sq);
-  PB_LAUNCH_CHECK();
-  k_sumsq<<<stream_grid(F), 256, 0, st>>>(gb_enc, F, &sc->gnorm_sq);
-  PB_LAUNCH_CHECK();
-  k_sumsq<<<1, 256, 0, st>>>(gb_dec, d, &sc->gnorm_sq);
-  PB_LAUNCH_CHECK();
-  k_grad_finish<<<1, 1, 0, st>>>(sc, max_grad_norm, 1.f / ((float)rows * (float)d), 1.f / (float)rows);
-  PB_LAUNCH_CHECK();
-  return PB_OK;
-}
-
 extern "C" int pb_sae_ghost_gather(const float* hidden_pre, const int32_t* dead_idx, int32_t nd, int32_t rows, int32_t F, float* E, int32_t ldE,
                                    pb_stream_t stream) {
   PB_CHECK_ARG(hidden_pre && E && (nd == 0 || dead_idx) && nd >= 0 && ldE >= nd && rows >= 0, "pb_sae_ghost_gather: bad arguments");

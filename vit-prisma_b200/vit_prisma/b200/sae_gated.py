@@ -21,8 +21,8 @@ import torch
 
 from . import _lib as L
 from . import ops
-from .sae_dense import _gemm_impl, _p, colsum, gemm32, gemv_rows, transpose
-from .sae_engine import SaeStepEngine, _need_cuda, _stream
+from .sae_dense import SaeDenseStepEngine, _dense_loss, colsum, transpose
+from .sae_engine import _need_cuda, _stream
 
 i32, f32, vp = C.c_int32, C.c_float, C.c_void_p
 
@@ -35,32 +35,27 @@ L.register_signatures({
 })
 
 
-class SaeGatedStepEngine(SaeStepEngine):
-    """Parameters: W_encT [F,d] (feature-major view of W_enc), W_dec [F,d], b_gate, r_mag, b_mag [F], b_dec [d]."""
+class SaeGatedStepEngine(SaeDenseStepEngine):
+    """Parameters: W_encT [F,d] (feature-major view of W_enc), W_dec [F,d], b_gate, r_mag, b_mag [F], b_dec [d].
+    aux = [sum_f colsum(pi_act) ||W_dec[f]||, sum (via - sae_in)^2, -, -]."""
 
     def __init__(self, W_encT: torch.Tensor, W_dec: torch.Tensor, b_gate: torch.Tensor, r_mag: torch.Tensor, b_mag: torch.Tensor,
                  b_dec: torch.Tensor, l1_coefficient: float, **kw):
-        kw["encoder"] = "dense"
-        super().__init__(W_encT, W_dec, b_gate, b_dec, k=1, **kw)     # b_gate rides in the b_enc slot of pb_sae_adam
+        # b_gate rides in the b_enc slot of pb_sae_adam
+        super().__init__(W_encT, W_dec, b_gate, b_dec, k=1, l1_coefficient=l1_coefficient, **kw)
         _need_cuda(r_mag, b_mag)
         self.b_gate, self.r_mag, self.b_mag = b_gate, r_mag, b_mag
-        self.l1_coefficient = float(l1_coefficient)
-        dev = W_dec.device
-        z = lambda n: torch.zeros(n, device=dev)  # noqa: E731
+        z = lambda n: torch.zeros(n, device=W_dec.device)  # noqa: E731
         self.m_r, self.v_r, self.m_bm, self.v_bm = z(self.F), z(self.F), z(self.F), z(self.F)
         self.gr_mag, self.gb_mag, self.dsum, self.piact_colsum, self.wnorm = z(self.F), z(self.F), z(self.F), z(self.F), z(self.F)
-        self.aux = torch.zeros(4, device=dev)                          # [sum_f colsum(pi_act) ||W_dec[f]||, sum (via - sae_in)^2, -, -]
-        self._zero_idx = torch.zeros(1, dtype=torch.int32, device=dev)
 
     # ------------------------------------------------------------------ forward pieces (shared by training and inference)
     def _forward(self, x: torch.Tensor, want_out: bool, training: bool):
         lib, st = L.get_lib(), _stream()
         rows, d, F = x.shape[0], self.d, self.F
-        self._ensure_rows(rows)
-        L.check(lib.pb_sae_prep(x.data_ptr(), self.b_dec.data_ptr(), self.sae_in.data_ptr(), self.sae_in_lo.data_ptr(), self.mu.data_ptr(),
-                                self.sd.data_ptr(), self.xsum.data_ptr(), rows, d, self.norm_mode, st), "pb_sae_prep")
-        self.scalars.zero_(); self.aux.zero_(); self.fired.zero_(); self.piact_colsum.zero_()
-        gemm32(self.sae_in, self.sae_in_lo, self.W_encT, self.W_encT_lo, self.b_gate, out0=self.hidden_pre)        # pi
+        self._prep(x)
+        self.piact_colsum.zero_()
+        self.gemm32(self.sae_in, self.sae_in_lo, self.W_encT, self.W_encT_lo, self.b_gate, out0=self.hidden_pre)   # pi
         dev = x.device
         acts, pi_act = torch.empty(rows, F, device=dev), torch.empty(rows, F, device=dev)
         acts_lo, pi_act_lo = torch.empty(rows, F, device=dev), torch.empty(rows, F, device=dev)
@@ -68,16 +63,15 @@ class SaeGatedStepEngine(SaeStepEngine):
                                  acts.data_ptr(), acts_lo.data_ptr(), pi_act.data_ptr(), pi_act_lo.data_ptr(), self.fired.data_ptr(),
                                  self.piact_colsum.data_ptr(), self.scalars.data_ptr(), rows, F, st), "pb_gated_fwd")
         WdT, WdT_lo = transpose(self.W_dec)                           # [d, F]: K-major B operand of both decoder products
-        out_n, _ = gemm32(acts, acts_lo, WdT, WdT_lo, self.b_dec)
-        via, _ = gemm32(pi_act, pi_act_lo, WdT, WdT_lo, self.b_dec)   # via-gate reconstruction (:786-787)
-        L.check(lib.pb_sae_dense_loss(x.data_ptr(), out_n.data_ptr(), self.mu.data_ptr(), self.sd.data_ptr(), self.xsum.data_ptr(),
-                                      self.sae_out.data_ptr() if want_out else None, self.g.data_ptr() if training else None, None,
-                                      self.scalars.data_ptr(), rows, 0, d, self.norm_mode, st), "pb_sae_dense_loss")
+        out_n, _ = self.gemm32(acts, acts_lo, WdT, WdT_lo, self.b_dec)
+        via, _ = self.gemm32(pi_act, pi_act_lo, WdT, WdT_lo, self.b_dec)   # via-gate reconstruction (:786-787)
+        _dense_loss(x, out_n, self.xsum, self.mu, self.sd, self.norm_mode, sae_out=self.sae_out if want_out else None,
+                    g=self.g if training else None, scalars=self.scalars)
         ga = torch.empty(rows, d, device=dev)
         L.check(lib.pb_gated_aux(via.data_ptr(), self.sae_in.data_ptr(), ga.data_ptr(), self.aux[1:].data_ptr(), rows, d, st), "pb_gated_aux")
         L.check(lib.pb_row_norms(self.W_dec.data_ptr(), self.wnorm.data_ptr(), F, d, st), "pb_row_norms")
         self.last_acts = acts
-        return acts, acts_lo, pi_act, pi_act_lo, ga
+        return acts, pi_act, ga
 
     @torch.no_grad()
     def forward_losses(self, x: torch.Tensor, want_out: bool = True) -> torch.Tensor:
@@ -85,8 +79,7 @@ class SaeGatedStepEngine(SaeStepEngine):
         _need_cuda(x)
         x = x.contiguous().float()
         lib, st = L.get_lib(), _stream()
-        with _gemm_impl(self.gemm_impl):
-            acts, _, _, _, _ = self._forward(x, want_out, training=False)
+        acts, _, _ = self._forward(x, want_out, training=False)
         # l1 value without touching any gradient buffer: sum_f colsum(pi_act)[f] * ||W_dec[f]||
         scratch = torch.zeros(self.F, self.d, device=x.device) if not hasattr(self, "_l1_scratch") else self._l1_scratch
         self._l1_scratch = scratch
@@ -100,49 +93,31 @@ class SaeGatedStepEngine(SaeStepEngine):
                          want_out: bool = False) -> torch.Tensor:
         _need_cuda(x)
         x = x.contiguous().float()
-        with _gemm_impl(self.gemm_impl):
-            return self._train_step(x, float(lr), since_fired, act_freq, want_out)
-
-    def _train_step(self, x, lr, since_fired, act_freq, want_out) -> torch.Tensor:
         lib, st = L.get_lib(), _stream()
         rows, d, F = x.shape[0], self.d, self.F
         self.step_count += 1
-        acts, acts_lo, pi_act, pi_act_lo, ga = self._forward(x, want_out, training=True)
+        acts, pi_act, ga = self._forward(x, want_out, training=True)
         l1_grad = self.l1_coefficient / rows
         Wd_lo = ops.split_tf32(self.W_dec)
-        D, _ = gemm32(self.g, None, self.W_dec, Wd_lo)               # d_acts = g @ W_dec^T, becomes D in place
-        d_pia, _ = gemm32(ga, None, self.W_dec, Wd_lo)
-        D_lo = torch.empty_like(D)
-        L.check(lib.pb_gated_bwd(D.data_ptr(), D_lo.data_ptr(), d_pia.data_ptr(), self.hidden_pre.data_ptr(), self.b_gate.data_ptr(),
+        D, _ = self.gemm32(self.g, None, self.W_dec, Wd_lo)          # d_acts = g @ W_dec^T, becomes D in place
+        d_pia, _ = self.gemm32(ga, None, self.W_dec, Wd_lo)
+        # no tf32 plane of D: the transpose for gW_encT makes the one its product reads
+        L.check(lib.pb_gated_bwd(D.data_ptr(), None, d_pia.data_ptr(), self.hidden_pre.data_ptr(), self.b_gate.data_ptr(),
                                  self.r_mag.data_ptr(), self.b_mag.data_ptr(), self.wnorm.data_ptr(), l1_grad, self.gb_enc.data_ptr(),
                                  self.gb_mag.data_ptr(), self.gr_mag.data_ptr(), self.dsum.data_ptr(), rows, F, st), "pb_gated_bwd")
         del d_pia
         # gW_dec = acts^T @ g + pi_act^T @ ga (+ L1 rows); the second product accumulates through the residual epilogue
-        gT, gT_lo = transpose(self.g)
-        gaT, gaT_lo = transpose(ga)
-        actsT, actsT_lo = transpose(acts)
-        first, _ = gemm32(actsT, actsT_lo, gT, gT_lo)
-        del actsT, actsT_lo
-        piT, piT_lo = transpose(pi_act)
-        if self.gemm_impl == L.GEMM_SIMT:
-            ops.gemm(piT, gaT, None, residual=first, out1=self.gW_dec, want_pre=False, impl=L.GEMM_SIMT)
-        else:
-            ops.gemm(piT, gaT, None, residual=first, out1=self.gW_dec, want_pre=False, a_lo=piT_lo, w_lo=gaT_lo)
-        del piT, piT_lo, first
+        self._at_b(pi_act, ga, out=self.gW_dec, residual=self._at_b(acts, self.g))
         L.check(lib.pb_gated_l1_rows(self.gW_dec.data_ptr(), self.W_dec.data_ptr(), self.piact_colsum.data_ptr(), self.wnorm.data_ptr(),
                                      l1_grad, self.aux.data_ptr(), F, d, st), "pb_gated_l1_rows")
-        # gW_enc^T = D^T @ sae_in
-        DT, DT_lo = transpose(D)
-        sinT, sinT_lo = transpose(self.sae_in)
-        gemm32(DT, DT_lo, sinT, sinT_lo, out0=self.gW_encT)
+        self._at_b(D, self.sae_in, out=self.gW_encT)                 # gW_enc^T = D^T @ sae_in
         # gb_dec = colsum(g) + 2 colsum(ga) - colsum(D) @ W_enc^T      (decoder bias twice, sae_in = xn - b_dec in the aux target and the encoder)
         colsum(self.g, out=self.gb_dec)
-        sc = lib.pb_scatter_add_rows
-        L.check(sc(self.gb_dec.data_ptr(), self._zero_idx.data_ptr(), 1, d, colsum(ga).data_ptr(), 2.0, st), "pb_scatter_add_rows")
-        L.check(sc(self.gb_dec.data_ptr(), self._zero_idx.data_ptr(), 1, d, gemv_rows(self.W_encT, self.dsum).data_ptr(), -1.0, st),
-                "pb_scatter_add_rows")
+        self._add_gb_dec(colsum(ga), 2.0)
+        self._gb_dec_through_sae_in(self.dsum, self.W_encT)
         # global norm over the six trained tensors -> clip coefficient -> Adam
-        self._clip_and_adam(x, lr, since_fired, act_freq, (self.gW_dec, self.gW_encT, self.gb_enc, self.gb_dec, self.gr_mag, self.gb_mag),
+        self._clip_and_adam(x, float(lr), since_fired, act_freq,
+                            (self.gW_dec, self.gW_encT, self.gb_enc, self.gb_dec, self.gr_mag, self.gb_mag),
                             ((self.r_mag, self.gr_mag, self.m_r, self.v_r), (self.b_mag, self.gb_mag, self.m_bm, self.v_bm)))
         return self.scalars
 

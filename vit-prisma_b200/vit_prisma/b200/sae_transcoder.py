@@ -19,10 +19,8 @@ from typing import Optional
 import torch
 
 from . import _lib as L
-from . import ops
-from .sae_dense import SaeDenseStepEngine, _gemm_impl, _p, colsum, gemm32, gemv_rows, transpose
-from .sae_engine import _need_cuda, _stream, topk_dense
-
+from .sae_dense import SaeDenseStepEngine, colsum, transpose
+from .sae_engine import _need_cuda, _stream
 
 
 class SaeTranscoderStepEngine(SaeDenseStepEngine):
@@ -47,40 +45,9 @@ class SaeTranscoderStepEngine(SaeDenseStepEngine):
 
     # ------------------------------------------------------------------ forward pieces
     def _forward(self, x: torch.Tensor, y: Optional[torch.Tensor], want_out: bool, training: bool):
-        lib, st = L.get_lib(), _stream()
-        rows, d, F = x.shape[0], self.d, self.F
-        self._ensure_rows(rows)
-        L.check(lib.pb_sae_prep(x.data_ptr(), self.b_dec.data_ptr(), self.sae_in.data_ptr(), self.sae_in_lo.data_ptr(), self.mu.data_ptr(),
-                                self.sd.data_ptr(), self.xsum.data_ptr(), rows, d, self.norm_mode, st), "pb_sae_prep")
-        self.scalars.zero_(); self.aux.zero_(); self.fired.zero_()
-        if self.activation == "relu":
-            acts = torch.empty(rows, F, device=x.device)
-            gemm32(self.sae_in, self.sae_in_lo, self.W_encT, self.W_encT_lo, self.b_enc, act="relu", out0=self.hidden_pre, out1=acts)
-        else:
-            gemm32(self.sae_in, self.sae_in_lo, self.W_encT, self.W_encT_lo, self.b_enc, out0=self.hidden_pre)
-            acts = topk_dense(self.hidden_pre, self.k)                       # zeros.scatter_(topk idx, relu(topk values))
-        L.check(lib.pb_sae_dense_stats(acts.data_ptr(), rows, F, self.fired.data_ptr(), self.aux.data_ptr(), self.scalars.data_ptr(), st),
-                "pb_sae_dense_stats")
-        WdT, WdT_lo = transpose(self.W_dec)
-        out_n, _ = gemm32(acts, None, WdT, WdT_lo, self.b_dec_out)
-        if self.W_skip is not None:                                           # + x @ W_skip^T: W_skip [d_out, d_in] is already K-major
-            x_lo = ops.split_tf32(x)
-            if self.gemm_impl == L.GEMM_SIMT:
-                _, out_n = ops.gemm(x, self.W_skip, None, residual=out_n, want_pre=False, impl=L.GEMM_SIMT)
-            else:
-                _, out_n = ops.gemm(x, self.W_skip, None, residual=out_n, want_pre=False, a_lo=x_lo, w_lo=ops.split_tf32(self.W_skip))
-        if y is not None:                                                      # loss against the TARGET activation, centred on its batch mean
+        if y is not None:                                     # loss against the TARGET activation, centred on its batch mean
             colsum(y, out=self.ysum)
-            L.check(lib.pb_sae_dense_loss(y.data_ptr(), out_n.data_ptr(), self.mu.data_ptr(), self.sd.data_ptr(), self.ysum.data_ptr(),
-                                          self.sae_out.data_ptr() if want_out else None, self.g.data_ptr() if training else None, None,
-                                          self.scalars.data_ptr(), rows, 0, d, self.norm_mode, st), "pb_sae_dense_loss")
-        elif want_out:                                                         # inference without a target: sae_out only
-            dummy = torch.zeros(8, device=x.device)
-            L.check(lib.pb_sae_dense_loss(x.data_ptr(), out_n.data_ptr(), self.mu.data_ptr(), self.sd.data_ptr(), self.xsum.data_ptr(),
-                                          self.sae_out.data_ptr(), None, None, dummy.data_ptr(), rows, 0, d, self.norm_mode, st),
-                    "pb_sae_dense_loss")
-        self.last_acts = acts
-        return acts
+        return self._dense_forward(x, y, self.ysum, self.b_dec_out, want_out, training, topk=self.activation == "topk", skip=self.W_skip)
 
     @torch.no_grad()
     def forward_losses(self, x: torch.Tensor, y: Optional[torch.Tensor], want_out: bool = True) -> torch.Tensor:
@@ -88,8 +55,7 @@ class SaeTranscoderStepEngine(SaeDenseStepEngine):
         _need_cuda(x, y)
         x = x.contiguous().float()
         y = None if y is None else y.contiguous().float()
-        with _gemm_impl(self.gemm_impl):
-            acts = self._forward(x, y, want_out, training=False)
+        acts = self._forward(x, y, want_out, training=False)
         L.check(L.get_lib().pb_sae_clip_finish(self.scalars.data_ptr(), 0.0, x.shape[0], self.d, _stream()), "pb_sae_clip_finish")
         return acts
 
@@ -99,38 +65,21 @@ class SaeTranscoderStepEngine(SaeDenseStepEngine):
                               act_freq: Optional[torch.Tensor] = None, want_out: bool = False) -> torch.Tensor:
         _need_cuda(x, y)
         x, y = x.contiguous().float(), y.contiguous().float()
-        with _gemm_impl(self.gemm_impl):
-            return self._train_step_tc(x, y, float(lr), since_fired, act_freq, want_out)
-
-    def _train_step_tc(self, x, y, lr, since_fired, act_freq, want_out) -> torch.Tensor:
-        lib, st = L.get_lib(), _stream()
-        rows, d = x.shape[0], self.d
         self.step_count += 1
         acts = self._forward(x, y, want_out, training=True)
-        l1_grad = (self.l1_coefficient / rows) if self.activation != "topk" else 0.0       # TopK: no sparsity term (transcoder.py:96-100)
-        d_hid, _ = gemm32(self.g, None, self.W_dec, None)                    # d_acts = g @ W_dec^T
-        d_hid_lo = torch.empty_like(d_hid)
-        L.check(lib.pb_sae_dense_dhid(d_hid.data_ptr(), acts.data_ptr(), d_hid_lo.data_ptr(), l1_grad, d_hid.numel(), st), "pb_sae_dense_dhid")
-        gT, gT_lo = transpose(self.g)                                        # [d, rows]
-        actsT, actsT_lo = transpose(acts)
-        gemm32(actsT, actsT_lo, gT, gT_lo, out0=self.gW_dec)                 # gW_dec = acts^T @ g
-        del actsT, actsT_lo
-        dhT, dhT_lo = transpose(d_hid)
-        sinT, sinT_lo = transpose(self.sae_in)
-        gemm32(dhT, dhT_lo, sinT, sinT_lo, out0=self.gW_encT)                # gW_enc^T = d_hid^T @ sae_in
-        colsum(d_hid, out=self.gb_enc)
+        l1_grad = (self.l1_coefficient / x.shape[0]) if self.activation != "topk" else 0.0   # TopK: no sparsity term (transcoder.py:96-100)
+        gT = transpose(self.g)                                               # [d, rows]: gW_dec's operand, and gW_skip's
+        self._dense_backward(acts, l1_grad, gT)
         colsum(self.g, out=self.gb_dec_out)                                   # b_dec_out enters the output only
-        tmp = gemv_rows(self.W_encT, self.gb_enc)                             # b_dec enters through sae_in = norm(x) - b_dec only
         self.gb_dec.zero_()
-        L.check(lib.pb_scatter_add_rows(self.gb_dec.data_ptr(), self._zero_idx.data_ptr(), 1, d, tmp.data_ptr(), -1.0, st), "pb_scatter_add_rows")
+        self._gb_dec_through_sae_in(self.gb_enc, self.W_encT)                 # b_dec enters through sae_in = norm(x) - b_dec only
         grads = [self.gW_dec, self.gW_encT, self.gb_enc, self.gb_dec, self.gb_dec_out]
         extra = [(self.b_dec_out, self.gb_dec_out, self.m_bo, self.v_bo)]
         if self.W_skip is not None:
-            xT, xT_lo = transpose(x)                                         # [d, rows]
-            gemm32(gT, gT_lo, xT, xT_lo, out0=self.gW_skip)                  # gW_skip = g^T @ x   ([d_out, d_in], out += x @ W_skip^T)
+            self._at_b(gT, x, out=self.gW_skip)                              # gW_skip = g^T @ x   ([d_out, d_in], out += x @ W_skip^T)
             grads.append(self.gW_skip)
             extra.append((self.W_skip, self.gW_skip, self.m_sk, self.v_sk))
-        self._clip_and_adam(x, lr, since_fired, act_freq, grads, extra)
+        self._clip_and_adam(x, float(lr), since_fired, act_freq, grads, extra)
         return self.scalars
 
     def loss_terms(self, rows: int) -> dict:
