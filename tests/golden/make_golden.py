@@ -27,6 +27,17 @@ TINY_A = dict(n_layers=2, d_model=32, d_head=8, n_heads=4, d_mlp=64, patch_size=
 TINY_B = dict(n_layers=2, d_model=24, d_head=8, n_heads=2, d_mlp=40, patch_size=8, image_size=32, n_channels=3,
               n_classes=7, eps=1e-6, activation_name="quick_gelu", normalization_type="LNPre", use_cls_token=False,
               layer_norm_pre=False, normalize_output=False, return_type="pre_logits", classification_type="gaap")
+# c: LayerNormPre in front of the blocks, cls pooling without a cls token (fp32: unscaled attention scores, which in
+#    bf16 are ~0.25 per ulp and put the reference's own bf16 run beyond any flat bar);
+# d: gaap pooling with a cls token and a normalised pre_logits output.  The activation differs per fixture.
+TINY_C = dict(n_layers=2, d_model=32, d_head=8, n_heads=4, d_mlp=48, patch_size=8, image_size=32, n_channels=3,
+              n_classes=9, eps=1e-5, normalization_type="LNPre", use_cls_token=False, layer_norm_pre=True,
+              normalize_output=True, return_type="class_logits", classification_type="cls")
+TINY_D = dict(n_layers=2, d_model=24, d_head=8, n_heads=3, d_mlp=56, patch_size=16, image_size=48, n_channels=3,
+              n_classes=5, eps=1e-6, normalization_type="LN", use_cls_token=True, layer_norm_pre=False,
+              normalize_output=True, return_type="pre_logits", classification_type="gaap")
+TINY_OVERRIDE = {("c", "fp32"): dict(activation_name="gelu_new", use_attn_scale=False), ("c", "bf16"): dict(activation_name="gelu_fast"),
+                 ("d", "fp32"): dict(activation_name="silu"), ("d", "bf16"): dict(activation_name="relu")}
 
 
 def ref_model(cfg: dict, dtype=torch.float32):
@@ -47,8 +58,9 @@ def images(batch, cfg, seed=0):
 
 
 def make_vit():
-    for tag, cfg in (("a", TINY_A), ("b", TINY_B)):
+    for tag, base in (("a", TINY_A), ("b", TINY_B), ("c", TINY_C), ("d", TINY_D)):
         for dtype, dname in ((torch.float32, "fp32"), (torch.bfloat16, "bf16")):
+            cfg = dict(base, **TINY_OVERRIDE.get((tag, dname), {}))
             model, shapes = ref_model(cfg, dtype)
             x = images(3, cfg).to(dtype)
             with torch.no_grad():

@@ -16,7 +16,7 @@ def _images(batch, cfg, seed=0):
     return torch.randn(batch, cfg["n_channels"], cfg["image_size"], cfg["image_size"], generator=g)
 
 
-@pytest.mark.parametrize("tag", ["a", "b"])
+@pytest.mark.parametrize("tag", ["a", "b", "c", "d"])
 @pytest.mark.parametrize("dname", ["fp32", "bf16"])
 def test_oracle_matches_reference_tiny(tag, dname):
     gold = load_golden(f"vit_tiny_{tag}_{dname}.pt")

@@ -48,7 +48,7 @@ def _model(cfg, dtype, seed=1234):
     return model, shapes
 
 
-@pytest.mark.parametrize("tag", ["a", "b"])
+@pytest.mark.parametrize("tag", ["a", "b", "c", "d"])
 @pytest.mark.parametrize("dname", ["fp32", "bf16"])
 @pytest.mark.parametrize("route", ["fused", "hooked"])
 def test_tiny_matches_reference_golden(tag, dname, route, monkeypatch):
