@@ -246,7 +246,8 @@ PB_API int pb_text_forward(const PbTextForward* f, pb_stream_t stream);
 /* ------------------------------------------------------- TopK SAE training step
  * Stands in for StandardSparseAutoencoder.forward + VisionSAETrainer.train_step
  * (sae/sae.py:557-645, 144-149, 275-297; sae/train_sae.py:278-411) with activation_fn_str == "topk".
- * All buffers fp32 unless noted; F = d_sae, d = d_in.  The encoder is stored feature-major:
+ * All buffers fp32 unless noted; F = d_sae, d = d_in (d % 4 == 0, d <= 8192: one warp per row up to 1536, one CTA per
+ * row past it; anything else is refused with PB_EUNSUPPORTED before any launch).  The encoder is stored feature-major:
  * W_encT [F][d] (the module's W_enc [d,F] parameter is a transposed view of the same memory).
  * One step = pb_sae_prep -> pb_gemm (hidden_pre = sae_in @ W_encT^T + b_enc) -> pb_sae_topk ->
  *            pb_sae_decode -> pb_sae_backward -> pb_sae_adam, all on one stream, no host sync.      */

@@ -405,6 +405,7 @@ extern "C" int pb_p2p_adam_allgather(const PbP2PStep* s, pb_stream_t stream) {
   PB_CHECK_ARG(s->m_dec && s->v_dec && s->m_enc && s->v_enc && s->m_be && s->v_be && s->m_bd && s->v_bd && s->scalars && s->b_dec,
                "pb_p2p_adam_allgather: optimizer state missing");
   PB_CHECK_ARG(s->step >= 1, "pb_p2p_adam_allgather: step counter starts at 1");
+  PB_CHECK_ARG(chunks_for(s->d) > 0, "pb_p2p_adam_allgather: d_in=%d unsupported by the data-parallel optimizer (needs d %% 4 == 0 and d <= 1536)", s->d);
   cudaStream_t st = (cudaStream_t)stream;
   const int per = s->F / s->world, f0 = s->rank * per, f1 = f0 + per;
   const AdamHyper h = adam_hyper(s->lr, s->beta1, s->beta2, s->adam_eps, s->step);

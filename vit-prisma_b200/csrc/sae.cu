@@ -946,6 +946,514 @@ __global__ void __launch_bounds__(256) k_unit_rows(float* __restrict__ W, float*
 }
 
 // =============================================================================================
+// 8. wide rows (1536 < d <= 8192).  The row kernels above hold a d-row in one warp's registers, which ends at 384 float4 per row.
+// Here a row belongs to the SAE_WIDE_THREADS threads of a CTA (CtaRow, sae_optim.cuh), each holding CHUNKS <= 8 float4, and the
+// sums over the row go through shared memory.  The per-feature gradients, whose outputs only add up over a feature's entry list,
+// keep one warp per feature and walk d in column slices of SAE_SLICE_VEC float4 instead: the work item is (feature, slice).
+// =============================================================================================
+template <int CHUNKS>
+__global__ void __launch_bounds__(SAE_WIDE_THREADS) k_sae_prep_wide(const float* __restrict__ x, const float* __restrict__ b_dec,
+                                                                    float* __restrict__ sae_in, float* __restrict__ sae_in_lo,
+                                                                    __half* __restrict__ sae_in16, float* __restrict__ mu_out,
+                                                                    float* __restrict__ std_out, int d, int norm_mode, float eps) {
+  pb_pdl();
+  __shared__ float red[SAE_WIDE_WARPS];
+  const CtaRow rw{red};
+  const int t = threadIdx.x, row = blockIdx.x;             // one row per CTA
+  const int nvec = d >> 2;
+  const float* xr = x + (int64_t)row * d;
+  float v[CHUNKS][4];
+  float sum = 0.f;
+#pragma unroll
+  for (int i = 0; i < CHUNKS; ++i) {
+    const int c4 = i * SAE_WIDE_THREADS + t;
+    if (c4 < nvec) { ld4(xr + 4 * c4, v[i]); sum += (v[i][0] + v[i][1]) + (v[i][2] + v[i][3]); }
+    else v[i][0] = v[i][1] = v[i][2] = v[i][3] = 0.f;
+  }
+  float mu = 0.f, inv = 1.f, sd = 1.f;
+  if (norm_mode == 1) {  // layer_norm
+    mu = rw.sum(sum) / (float)d;
+    float sq = 0.f;
+#pragma unroll
+    for (int i = 0; i < CHUNKS; ++i) {
+      const int c4 = i * SAE_WIDE_THREADS + t;
+      if (c4 < nvec) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) { v[i][j] -= mu; sq += v[i][j] * v[i][j]; }
+      }
+    }
+    sd = sqrtf(rw.sum(sq) / (float)(d - 1));
+  } else if (norm_mode == 2) {  // constant_norm_rescale
+    float sq = 0.f;
+#pragma unroll
+    for (int i = 0; i < CHUNKS; ++i)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) sq += v[i][j] * v[i][j];
+    sd = sqrtf(rw.sum(sq)) / sqrtf((float)d);
+    inv = 1.f / sd;
+  }
+  if (t == 0) {
+    if (mu_out) mu_out[row] = mu;
+    if (std_out) std_out[row] = sd;
+  }
+#pragma unroll
+  for (int i = 0; i < CHUNKS; ++i) {
+    const int c4 = i * SAE_WIDE_THREADS + t;
+    if (c4 < nvec) {
+      float bd[4], o[4], lo[4];
+      ld4(b_dec + 4 * c4, bd);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        o[j] = (norm_mode == 1 ? v[i][j] / (sd + eps) : v[i][j] * inv) - bd[j];
+        lo[j] = tf32_lo(o[j]);
+      }
+      st4(sae_in + (int64_t)row * d + 4 * c4, o);
+      if (sae_in_lo) st4(sae_in_lo + (int64_t)row * d + 4 * c4, lo);
+      if (sae_in16) {
+        float unused = 0.f;
+        *reinterpret_cast<uint2*>(sae_in16 + (int64_t)row * d + 4 * c4) = f16x4(o, unused);
+      }
+    }
+  }
+}
+
+// decode + loss + dval of one token per CTA (k_sae_decode's arithmetic).  The dval dot products are per-warp partials over the
+// warp's columns, [warp][j] in shared memory, summed in warp order once all k are done.
+constexpr int SAE_WIDE_MAX_K = 256;
+template <int CHUNKS>
+__global__ void __launch_bounds__(SAE_WIDE_THREADS) k_sae_decode_wide(const float* __restrict__ x, const float* __restrict__ xsum,
+                                                                      const float* __restrict__ mu, const float* __restrict__ sd,
+                                                                      const int* __restrict__ idx, const float* __restrict__ val,
+                                                                      const float* __restrict__ W_dec, const float* __restrict__ b_dec,
+                                                                      float* __restrict__ sae_out, float* __restrict__ g_out,
+                                                                      float* __restrict__ dval, SaeScalars* __restrict__ sc, int d, int k,
+                                                                      int norm_mode, int training, float inv_rows) {
+  pb_pdl();
+  __shared__ float red[SAE_WIDE_WARPS];
+  __shared__ float dots[SAE_WIDE_WARPS][SAE_WIDE_MAX_K];
+  const CtaRow rw{red};
+  const int t = threadIdx.x, lane = t & 31, warp = t >> 5, row = blockIdx.x;
+  const int nvec = d >> 2;
+  const int* ir = idx + (int64_t)row * k;
+  const float* vr = val + (int64_t)row * k;
+  float acc[CHUNKS][4];
+#pragma unroll
+  for (int i = 0; i < CHUNKS; ++i) {
+    const int c4 = i * SAE_WIDE_THREADS + t;
+    if (c4 < nvec) ld4(b_dec + 4 * c4, acc[i]);
+    else acc[i][0] = acc[i][1] = acc[i][2] = acc[i][3] = 0.f;
+  }
+  float pos_part = 0.f;
+  for (int j0 = 0; j0 < k; j0 += 32) {
+    const int jn = min(32, k - j0);
+    const int my_i = lane < jn ? ir[j0 + lane] : 0;
+    const float my_a = lane < jn ? fmaxf(vr[j0 + lane], 0.f) : 0.f;
+    pos_part += (float)__popc(__ballot_sync(0xffffffffu, my_a > 0.f));
+#pragma unroll 4
+    for (int j = 0; j < jn; ++j) {
+      const float a = __shfl_sync(0xffffffffu, my_a, j);
+      const float* wr = W_dec + (int64_t)__shfl_sync(0xffffffffu, my_i, j) * d;
+#pragma unroll
+      for (int i = 0; i < CHUNKS; ++i) {
+        const int c4 = i * SAE_WIDE_THREADS + t;
+        if (c4 < nvec) {
+          float w[4];
+          ld4(wr + 4 * c4, w);
+#pragma unroll
+          for (int q = 0; q < 4; ++q) acc[i][q] = fmaf(a, w[q], acc[i][q]);
+        }
+      }
+    }
+  }
+  const float m = norm_mode ? mu[row] : 0.f;
+  const float s = norm_mode ? sd[row] : 1.f;
+  float nsq = 0.f;
+  float e[CHUNKS][4];
+#pragma unroll
+  for (int i = 0; i < CHUNKS; ++i) {
+    const int c4 = i * SAE_WIDE_THREADS + t;
+    if (c4 < nvec) {
+      float xv[4], xs[4], o[4];
+      ld4(x + (int64_t)row * d + 4 * c4, xv);
+      ld4(xsum + 4 * c4, xs);
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        o[q] = norm_mode == 1 ? acc[i][q] * s + m : (norm_mode == 2 ? acc[i][q] * s : acc[i][q]);
+        const float xc = xv[q] - xs[q] * inv_rows;
+        nsq += xc * xc;
+        e[i][q] = o[q] - xv[q];
+      }
+      if (sae_out) st4(sae_out + (int64_t)row * d + 4 * c4, o);
+    } else {
+      e[i][0] = e[i][1] = e[i][2] = e[i][3] = 0.f;
+    }
+  }
+  const float nf = sqrtf(rw.sum(nsq));
+  float esq = 0.f;
+#pragma unroll
+  for (int i = 0; i < CHUNKS; ++i)
+#pragma unroll
+    for (int q = 0; q < 4; ++q) esq += e[i][q] * e[i][q];
+  const float loss = rw.sum(esq) / nf;
+  if (training) {
+    const float gs = 2.f * s * inv_rows / ((float)d * nf);
+#pragma unroll
+    for (int i = 0; i < CHUNKS; ++i) {
+      const int c4 = i * SAE_WIDE_THREADS + t;
+#pragma unroll
+      for (int q = 0; q < 4; ++q) e[i][q] *= gs;
+      if (c4 < nvec) st4(g_out + (int64_t)row * d + 4 * c4, e[i]);
+    }
+    for (int j0 = 0; j0 < k; j0 += 32) {
+      const int jn = min(32, k - j0);
+      const int my_i = lane < jn ? ir[j0 + lane] : 0;
+#pragma unroll 4
+      for (int j = 0; j < jn; ++j) {
+        const float* wr = W_dec + (int64_t)__shfl_sync(0xffffffffu, my_i, j) * d;
+        float dot = 0.f;
+#pragma unroll
+        for (int i = 0; i < CHUNKS; ++i) {
+          const int c4 = i * SAE_WIDE_THREADS + t;
+          if (c4 < nvec) {
+            float w[4];
+            ld4(wr + 4 * c4, w);
+#pragma unroll
+            for (int q = 0; q < 4; ++q) dot = fmaf(e[i][q], w[q], dot);
+          }
+        }
+        dot = warp_sum(dot);
+        if (lane == 0) dots[warp][j0 + j] = dot;
+      }
+    }
+    __syncthreads();
+    for (int j = t; j < k; j += SAE_WIDE_THREADS) {
+      float dot = 0.f;
+#pragma unroll
+      for (int w = 0; w < SAE_WIDE_WARPS; ++w) dot += dots[w][j];
+      dval[(int64_t)row * k + j] = vr[j] > 0.f ? dot : 0.f;     // ReLU backward on the TopK support
+    }
+  }
+  if (t == 0) {
+    atomicAdd(&sc->loss_sum, loss);
+    atomicAdd(&sc->pos_count, (unsigned)pos_part);
+  }
+}
+
+// per-feature gradients over column slices (k_sae_grads' arithmetic, one warp per (feature, slice) work item).  Items are numbered
+// slice-major (item = s * F + f), so the items a warp claims in a row mostly share a slice; its register partial of gbdec2 covers
+// one slice and goes to the CTA's shared partial when the slice changes.  gb_enc, fired, gb_enc^2 and the hot-feature queue
+// belong to slice 0.
+constexpr int SAE_SLICE_CHUNKS = 8;                          // float4 per lane of a slice
+constexpr int SAE_SLICE_VEC = 32 * SAE_SLICE_CHUNKS;         // float4 per slice (1024 columns)
+
+__device__ __forceinline__ void flush_bd_slice(float (&bd)[SAE_SLICE_CHUNKS][4], float* sm_bd, int s, int nvec) {
+  const int lane = threadIdx.x & 31;
+#pragma unroll
+  for (int i = 0; i < SAE_SLICE_CHUNKS; ++i) {
+    const int c4 = s * SAE_SLICE_VEC + i * 32 + lane;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      if (c4 < nvec && bd[i][q] != 0.f) atomicAdd(&sm_bd[4 * c4 + q], bd[i][q]);
+      bd[i][q] = 0.f;
+    }
+  }
+}
+
+__global__ void __launch_bounds__(256) k_sae_grads_wide(const int* __restrict__ off, int* __restrict__ entries, const float* __restrict__ val,
+                                                        const float* __restrict__ dval, const float* __restrict__ g,
+                                                        const float* __restrict__ sae_in, const float* __restrict__ W_encT,
+                                                        float* __restrict__ gW_dec, float* __restrict__ gW_encT, float* __restrict__ gb_enc,
+                                                        float* __restrict__ gbdec2, float* __restrict__ fired, SaeScalars* __restrict__ sc,
+                                                        int F, int d, int k, int nsl, SaeWorkHeader* __restrict__ work,
+                                                        int* __restrict__ work_feats, int* __restrict__ work_chunks) {
+  pb_pdl();
+  extern __shared__ __align__(16) float sm_bd[];  // [d] per-CTA partial of gbdec2
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+  const int nvec = d >> 2;
+  for (int c = threadIdx.x; c < d; c += blockDim.x) sm_bd[c] = 0.f;
+  __syncthreads();
+  float nsq = 0.f;
+  float bd[SAE_SLICE_CHUNKS][4];
+#pragma unroll
+  for (int i = 0; i < SAE_SLICE_CHUNKS; ++i) bd[i][0] = bd[i][1] = bd[i][2] = bd[i][3] = 0.f;
+  int bd_s = 0;
+  const int n_items = F * nsl;
+  for (;;) {
+    int ibase = 0;
+    if (lane == 0) ibase = atomicAdd(&work->next_f, SAE_CLAIM);
+    ibase = __shfl_sync(0xffffffffu, ibase, 0);
+    if (ibase >= n_items) break;
+    for (int item = ibase; item < min(n_items, ibase + SAE_CLAIM); ++item) {
+      const int s = item / F, f = item - s * F;
+      if (s != bd_s) { flush_bd_slice(bd, sm_bd, bd_s, nvec); bd_s = s; }
+      const int cbase = s * SAE_SLICE_VEC;
+      const int e0 = off[f], e1 = off[f + 1];
+      const int len = e1 - e0;
+      if (len > SAE_LONG_LIST) {       // hot feature: every slice zeroes its columns, slice 0 queues the list for k_sae_grads_long_wide
+#pragma unroll
+        for (int i = 0; i < SAE_SLICE_CHUNKS; ++i) {
+          const int c4 = cbase + i * 32 + lane;
+          if (c4 < nvec) {
+            const float z4[4] = {0.f, 0.f, 0.f, 0.f};
+            st4(gW_dec + (int64_t)f * d + 4 * c4, z4);
+            st4(gW_encT + (int64_t)f * d + 4 * c4, z4);
+          }
+        }
+        if (s == 0) {
+          const int nchunks = (len + SAE_LONG_CHUNK - 1) / SAE_LONG_CHUNK;
+          int base = 0, lslot = 0;
+          if (lane == 0) {
+            gb_enc[f] = 0.f;
+            fired[f] = 0.f;
+            base = atomicAdd(&work->n_chunks, nchunks);
+            lslot = atomicAdd(&work->n_long, 1);
+            work_feats[lslot] = f;
+          }
+          base = __shfl_sync(0xffffffffu, base, 0);
+          for (int c = lane; c < nchunks; c += 32) {
+            work_chunks[2 * (base + c)] = f;
+            work_chunks[2 * (base + c) + 1] = e0 + c * SAE_LONG_CHUNK;
+          }
+        }
+        continue;
+      }
+      // the list (<= 32 entries) sorted by token index in the warp, as in k_sae_grads
+      int my_b = 0;
+      float my_a = 0.f, my_dp = 0.f;
+      {
+        const int mine = lane < len ? entries[e0 + lane] : 0x7fffffff;
+        int rank = 0;
+#pragma unroll
+        for (int j = 0; j < 32; ++j) rank += __shfl_sync(0xffffffffu, mine, j) < mine ? 1 : 0;
+        int src = 0;
+#pragma unroll
+        for (int j = 0; j < 32; ++j) src = (__shfl_sync(0xffffffffu, rank, j) == lane && j < len) ? j : src;
+        const int sorted = __shfl_sync(0xffffffffu, mine, src);
+        if (lane < len) {
+          my_b = sorted / k;
+          my_a = fmaxf(val[sorted], 0.f);
+          my_dp = dval[sorted];
+        }
+      }
+      float ad[SAE_SLICE_CHUNKS][4], ae[SAE_SLICE_CHUNKS][4];
+#pragma unroll
+      for (int i = 0; i < SAE_SLICE_CHUNKS; ++i) ad[i][0] = ad[i][1] = ad[i][2] = ad[i][3] = ae[i][0] = ae[i][1] = ae[i][2] = ae[i][3] = 0.f;
+      float gbe = 0.f;
+      const float npos = (float)__popc(__ballot_sync(0xffffffffu, my_a > 0.f));
+#pragma unroll 2
+      for (int j = 0; j < len; ++j) {
+        const float a = __shfl_sync(0xffffffffu, my_a, j), dp = __shfl_sync(0xffffffffu, my_dp, j);
+        const int b = __shfl_sync(0xffffffffu, my_b, j);
+        gbe += dp;
+        const float* gr = g + (int64_t)b * d;
+        const float* sr = sae_in + (int64_t)b * d;
+#pragma unroll
+        for (int i = 0; i < SAE_SLICE_CHUNKS; ++i) {
+          const int c4 = cbase + i * 32 + lane;
+          if (c4 < nvec) {
+            float gv[4], sv[4];
+            ld4(gr + 4 * c4, gv);
+            ld4(sr + 4 * c4, sv);
+#pragma unroll
+            for (int q = 0; q < 4; ++q) { ad[i][q] = fmaf(a, gv[q], ad[i][q]); ae[i][q] = fmaf(dp, sv[q], ae[i][q]); }
+          }
+        }
+      }
+#pragma unroll
+      for (int i = 0; i < SAE_SLICE_CHUNKS; ++i) {
+        const int c4 = cbase + i * 32 + lane;
+        if (c4 < nvec) {
+          st4(gW_dec + (int64_t)f * d + 4 * c4, ad[i]);
+          st4(gW_encT + (int64_t)f * d + 4 * c4, ae[i]);
+#pragma unroll
+          for (int q = 0; q < 4; ++q) nsq += ad[i][q] * ad[i][q] + ae[i][q] * ae[i][q];
+          if (gbe != 0.f) {
+            float w[4];
+            ld4(W_encT + (int64_t)f * d + 4 * c4, w);
+#pragma unroll
+            for (int q = 0; q < 4; ++q) bd[i][q] = fmaf(gbe, w[q], bd[i][q]);
+          }
+        }
+      }
+      if (lane == 0 && s == 0) {
+        gb_enc[f] = gbe;
+        fired[f] = npos;
+        nsq += gbe * gbe;
+      }
+    }
+  }
+  flush_bd_slice(bd, sm_bd, bd_s, nvec);
+  nsq = warp_sum(nsq);
+  __shared__ float red[8];
+  if (lane == 0) red[warp] = nsq;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float a = 0.f;
+    for (int i = 0; i < nw; ++i) a += red[i];
+    atomicAdd(&sc->gnorm_sq, a);
+  }
+  for (int c = threadIdx.x; c < d; c += blockDim.x)
+    if (sm_bd[c] != 0.f) atomicAdd(gbdec2 + c, sm_bd[c]);
+}
+
+// hot features over column slices: one warp per (chunk of SAE_LONG_CHUNK entries, slice), numbered slice-major
+__global__ void __launch_bounds__(256) k_sae_grads_long_wide(const int* __restrict__ off, const int* __restrict__ entries,
+                                                             const float* __restrict__ val, const float* __restrict__ dval,
+                                                             const float* __restrict__ g, const float* __restrict__ sae_in,
+                                                             const float* __restrict__ W_encT, float* __restrict__ gW_dec,
+                                                             float* __restrict__ gW_encT, float* __restrict__ gb_enc, float* __restrict__ gbdec2,
+                                                             float* __restrict__ fired, int d, int k, int nsl,
+                                                             const SaeWorkHeader* __restrict__ work, const int* __restrict__ work_chunks) {
+  pb_pdl();
+  extern __shared__ __align__(16) float sm_bd[];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+  const int nvec = d >> 2;
+  const int n_chunks = work->n_chunks;
+  if (n_chunks == 0) return;
+  for (int c = threadIdx.x; c < d; c += blockDim.x) sm_bd[c] = 0.f;
+  __syncthreads();
+  float bd[SAE_SLICE_CHUNKS][4];
+#pragma unroll
+  for (int i = 0; i < SAE_SLICE_CHUNKS; ++i) bd[i][0] = bd[i][1] = bd[i][2] = bd[i][3] = 0.f;
+  int bd_s = 0;
+  const int n_items = n_chunks * nsl;
+  for (int item = blockIdx.x * nw + warp; item < n_items; item += gridDim.x * nw) {
+    const int s = item / n_chunks, ci = item - s * n_chunks;
+    if (s != bd_s) { flush_bd_slice(bd, sm_bd, bd_s, nvec); bd_s = s; }
+    const int cbase = s * SAE_SLICE_VEC;
+    const int f = work_chunks[2 * ci], p0 = work_chunks[2 * ci + 1];
+    const int p1 = min(off[f + 1], p0 + SAE_LONG_CHUNK);
+    float ad[SAE_SLICE_CHUNKS][4], ae[SAE_SLICE_CHUNKS][4];
+#pragma unroll
+    for (int i = 0; i < SAE_SLICE_CHUNKS; ++i) ad[i][0] = ad[i][1] = ad[i][2] = ad[i][3] = ae[i][0] = ae[i][1] = ae[i][2] = ae[i][3] = 0.f;
+    const int n = p1 - p0;
+    int my_b = 0;
+    float my_a = 0.f, my_dp = 0.f;
+    if (lane < n) {
+      const int e = entries[p0 + lane];
+      my_b = e / k;
+      my_a = fmaxf(val[e], 0.f);
+      my_dp = dval[e];
+    }
+    float gbe = 0.f;
+    const float npos = (float)__popc(__ballot_sync(0xffffffffu, my_a > 0.f));
+#pragma unroll 2
+    for (int j = 0; j < n; ++j) {
+      const float a = __shfl_sync(0xffffffffu, my_a, j), dp = __shfl_sync(0xffffffffu, my_dp, j);
+      const int b = __shfl_sync(0xffffffffu, my_b, j);
+      gbe += dp;
+      const float* gr = g + (int64_t)b * d;
+      const float* sr = sae_in + (int64_t)b * d;
+#pragma unroll
+      for (int i = 0; i < SAE_SLICE_CHUNKS; ++i) {
+        const int c4 = cbase + i * 32 + lane;
+        if (c4 < nvec) {
+          float gv[4], sv[4];
+          ld4(gr + 4 * c4, gv);
+          ld4(sr + 4 * c4, sv);
+#pragma unroll
+          for (int q = 0; q < 4; ++q) { ad[i][q] = fmaf(a, gv[q], ad[i][q]); ae[i][q] = fmaf(dp, sv[q], ae[i][q]); }
+        }
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < SAE_SLICE_CHUNKS; ++i) {
+      const int c4 = cbase + i * 32 + lane;
+      if (c4 < nvec) {
+        atomicAdd(reinterpret_cast<float4*>(gW_dec + (int64_t)f * d + 4 * c4), make_float4(ad[i][0], ad[i][1], ad[i][2], ad[i][3]));
+        atomicAdd(reinterpret_cast<float4*>(gW_encT + (int64_t)f * d + 4 * c4), make_float4(ae[i][0], ae[i][1], ae[i][2], ae[i][3]));
+        if (gbe != 0.f) {
+          float w[4];
+          ld4(W_encT + (int64_t)f * d + 4 * c4, w);
+#pragma unroll
+          for (int q = 0; q < 4; ++q) bd[i][q] = fmaf(gbe, w[q], bd[i][q]);
+        }
+      }
+    }
+    if (lane == 0 && s == 0) {
+      atomicAdd(gb_enc + f, gbe);
+      atomicAdd(fired + f, npos);
+    }
+  }
+  flush_bd_slice(bd, sm_bd, bd_s, nvec);
+  __syncthreads();
+  for (int c = threadIdx.x; c < d; c += blockDim.x)
+    if (sm_bd[c] != 0.f) atomicAdd(gbdec2 + c, sm_bd[c]);
+}
+
+// the optimizer with one feature per CTA: sae_adam_feature over a CtaRow, then k_sae_adam_rows' bias / counter / norm-max epilogue
+template <int CHUNKS>
+__global__ void __launch_bounds__(SAE_WIDE_THREADS) k_sae_adam_rows_wide(float* __restrict__ W_dec, float* __restrict__ W_encT,
+                                                                         float* __restrict__ W_encT_lo, __half* __restrict__ W_encT16,
+                                                                         float* __restrict__ enc16_lo_max, float* __restrict__ b_enc,
+                                                                         const float* __restrict__ gW_dec, const float* __restrict__ gW_encT,
+                                                                         const float* __restrict__ gb_enc, float* __restrict__ m_dec,
+                                                                         float* __restrict__ v_dec, float* __restrict__ m_enc,
+                                                                         float* __restrict__ v_enc, float* __restrict__ m_be,
+                                                                         float* __restrict__ v_be, const float* __restrict__ fired,
+                                                                         float* __restrict__ since_fired, float* __restrict__ act_freq,
+                                                                         const SaeScalars* __restrict__ sc, AdamHyper h, int F, int d,
+                                                                         int renorm, float* __restrict__ enc_norm_max) {
+  __shared__ float red[SAE_WIDE_WARPS];
+  const CtaRow rw{red};
+  const int nvec = d >> 2;
+  const float clip = sc->clip_coef;
+  float enc_best = 0.f, enc_best_lo = 0.f, enc_best16 = 0.f;
+  for (int f = blockIdx.x; f < F; f += gridDim.x) {
+    const int64_t base = (int64_t)f * d;
+    float esq, elo, e16;
+    sae_adam_feature<CHUNKS>(W_dec + base, gW_dec + base, m_dec + base, v_dec + base, W_encT + base, gW_encT + base, m_enc + base,
+                             v_enc + base, clip, h, nvec, renorm, AdamRowsOut{W_dec, W_encT, W_encT_lo, W_encT16, base}, esq, elo, e16, rw);
+    if (enc_norm_max) { enc_best = fmaxf(enc_best, rw.sum(esq)); enc_best_lo = fmaxf(enc_best_lo, rw.sum(elo)); }
+    if (enc16_lo_max) enc_best16 = fmaxf(enc_best16, rw.sum(e16));
+    if (threadIdx.x == 0) {
+      float mm = m_be[f], vv = v_be[f];
+      b_enc[f] = adam_update(b_enc[f], gb_enc[f] * clip, mm, vv, h);
+      m_be[f] = mm;
+      v_be[f] = vv;
+      dead_feature_counters(since_fired, act_freq, f, fired[f], since_fired ? since_fired[f] : 0.f, act_freq ? act_freq[f] : 0.f);
+    }
+  }
+  if (enc_norm_max && threadIdx.x == 0 && enc_best > 0.f) {
+    atomicMax(reinterpret_cast<unsigned int*>(enc_norm_max), __float_as_uint(sqrtf(enc_best)));
+    atomicMax(reinterpret_cast<unsigned int*>(enc_norm_max) + 1, __float_as_uint(sqrtf(enc_best_lo)));
+  }
+  if (enc16_lo_max && threadIdx.x == 0) atomic_max_norm(enc16_lo_max, enc_best16);
+}
+
+template <int CHUNKS>
+__global__ void __launch_bounds__(SAE_WIDE_THREADS) k_unit_rows_wide(float* __restrict__ W, float* __restrict__ W_lo, int F, int d) {
+  __shared__ float red[SAE_WIDE_WARPS];
+  const CtaRow rw{red};
+  const int t = threadIdx.x, nvec = d >> 2;
+  for (int f = blockIdx.x; f < F; f += gridDim.x) {
+    float w[CHUNKS][4];
+    float nsq = 0.f;
+#pragma unroll
+    for (int i = 0; i < CHUNKS; ++i) {
+      const int c4 = i * SAE_WIDE_THREADS + t;
+      if (c4 < nvec) {
+        ld4(W + (int64_t)f * d + 4 * c4, w[i]);
+#pragma unroll
+        for (int q = 0; q < 4; ++q) nsq += w[i][q] * w[i][q];
+      }
+    }
+    const float nrm = sqrtf(rw.sum(nsq));
+#pragma unroll
+    for (int i = 0; i < CHUNKS; ++i) {
+      const int c4 = i * SAE_WIDE_THREADS + t;
+      if (c4 < nvec) {
+        float lo[4];
+#pragma unroll
+        for (int q = 0; q < 4; ++q) { w[i][q] = w[i][q] / nrm; lo[q] = tf32_lo(w[i][q]); }
+        st4(W + (int64_t)f * d + 4 * c4, w[i]);
+        if (W_lo) st4(W_lo + (int64_t)f * d + 4 * c4, lo);
+      }
+    }
+  }
+}
+
+// =============================================================================================
 // host side
 // =============================================================================================
 static int persistent_grid(int warps_per_cta, int items) {
@@ -960,11 +1468,17 @@ static int launch_prep(const float* x, const float* b_dec, float* sae_in, float*
   PB_CHECK_ARG(x && b_dec && sae_in && rows >= 0 && d > 0, "pb_sae_prep: bad arguments");
   PB_CHECK_ARG(norm_mode == 0 || (mu && sd), "pb_sae_prep: mu/std buffers required when normalising");
   PB_CHECK_ARG(!sae_in16 || ((uintptr_t)sae_in16 & 7) == 0, "pb_sae_prep16: sae_in16 must be 8-byte aligned");
+  const int ch = chunks_for(d), wch = wide_chunks_for(d);
+  if (ch < 0 && wch < 0) PB_SAE_D_UNSUPPORTED();
   if (rows == 0) return PB_OK;
   cudaStream_t st = (cudaStream_t)stream;
-  const int ch = chunks_for(d);
-  PB_DISPATCH_CHUNKS(ch, PB_LAUNCH_PDL(k_sae_prep<C_>, (rows + 7) / 8, 256, 0, st, x, b_dec, sae_in, sae_in_lo, sae_in16, mu, sd, rows, d, norm_mode,
-                                       1e-5f));
+  if (wch > 0) {
+    PB_DISPATCH_WIDE(wch, PB_LAUNCH_PDL(k_sae_prep_wide<C_>, rows, SAE_WIDE_THREADS, 0, st, x, b_dec, sae_in, sae_in_lo, sae_in16, mu, sd, d,
+                                        norm_mode, 1e-5f));
+  } else {
+    PB_DISPATCH_CHUNKS(ch, PB_LAUNCH_PDL(k_sae_prep<C_>, (rows + 7) / 8, 256, 0, st, x, b_dec, sae_in, sae_in_lo, sae_in16, mu, sd, rows, d, norm_mode,
+                                         1e-5f));
+  }
   if (xsum) {
     PB_CUDA(cudaMemsetAsync(xsum, 0, sizeof(float) * d, st));
     const int rpc = 8;
@@ -1071,12 +1585,21 @@ extern "C" int pb_sae_step_reset(const PbSaeStep* s, int32_t* fb_count, pb_strea
 extern "C" int pb_sae_decode(const PbSaeStep* s, pb_stream_t stream) {
   PB_CHECK_ARG(s && s->x && s->xsum && s->idx && s->val && s->W_dec && s->b_dec && s->scalars, "pb_sae_decode: missing pointers");
   PB_CHECK_ARG(!s->training || (s->g && s->dval), "pb_sae_decode: training needs g and dval buffers");
+  const int d = s->d, ch = chunks_for(d), wch = wide_chunks_for(d);
+  if (ch < 0 && wch < 0) PB_SAE_D_UNSUPPORTED();
+  PB_CHECK_ARG(wch < 0 || s->k <= SAE_WIDE_MAX_K, "pb_sae_decode: k=%d > %d unsupported at d_in > 1536", s->k, SAE_WIDE_MAX_K);
   if (s->rows == 0) return PB_OK;
   cudaStream_t st = (cudaStream_t)stream;
-  const int d = s->d, ch = chunks_for(d);
-  PB_DISPATCH_CHUNKS(ch, PB_LAUNCH_PDL(k_sae_decode<C_>, (s->rows + 7) / 8, 256, 0, st,
-      s->x, s->xsum, s->mu, s->sd, s->idx, s->val, s->W_dec, s->b_dec, s->sae_out, s->g, s->dval, (SaeScalars*)s->scalars, s->rows, d, s->k,
-      s->norm_mode, s->training, 1.f / (float)(s->global_rows > 0 ? s->global_rows : s->rows)));
+  const float inv_rows = 1.f / (float)(s->global_rows > 0 ? s->global_rows : s->rows);
+  if (wch > 0) {
+    PB_DISPATCH_WIDE(wch, PB_LAUNCH_PDL(k_sae_decode_wide<C_>, s->rows, SAE_WIDE_THREADS, 0, st, s->x, s->xsum, s->mu, s->sd, s->idx, s->val,
+                                        s->W_dec, s->b_dec, s->sae_out, s->g, s->dval, (SaeScalars*)s->scalars, d, s->k, s->norm_mode,
+                                        s->training, inv_rows));
+  } else {
+    PB_DISPATCH_CHUNKS(ch, PB_LAUNCH_PDL(k_sae_decode<C_>, (s->rows + 7) / 8, 256, 0, st,
+        s->x, s->xsum, s->mu, s->sd, s->idx, s->val, s->W_dec, s->b_dec, s->sae_out, s->g, s->dval, (SaeScalars*)s->scalars, s->rows, d, s->k,
+        s->norm_mode, s->training, inv_rows));
+  }
   if (!s->training) {  // inference: publish mse / l0 now (the training path does it in k_sae_finalize)
     k_sae_fwd_scalars<<<1, 1, 0, st>>>((SaeScalars*)s->scalars, 1.f / ((float)s->rows * (float)d), 1.f / (float)s->rows);
     PB_LAUNCH_CHECK();
@@ -1088,9 +1611,10 @@ extern "C" int pb_sae_backward(const PbSaeStep* s, pb_stream_t stream) {
   PB_CHECK_ARG(s && s->idx && s->val && s->dval && s->g && s->sae_in && s->W_encT && s->feat_count && s->csc_off && s->csc_cursor &&
                s->csc_entries && s->gW_dec && s->gW_encT && s->gb_enc && s->gb_dec && s->gcol && s->gbdec2 && s->fired && s->scalars,
                "pb_sae_backward: missing pointers");
+  const int d = s->d, F = s->F, ch = chunks_for(d), wch = wide_chunks_for(d);
+  if (ch < 0 && wch < 0) PB_SAE_D_UNSUPPORTED();
   if (s->rows == 0) return PB_OK;
   cudaStream_t st = (cudaStream_t)stream;
-  const int d = s->d, F = s->F, ch = chunks_for(d);
   {
     const int per = ((F + 1023) / 1024 + 3) / 4 * 4;
     PB_CHECK_ARG(per <= 128, "pb_sae_backward: d_sae=%d too large for the offset scan (max 131072)", F);
@@ -1117,12 +1641,21 @@ extern "C" int pb_sae_backward(const PbSaeStep* s, pb_stream_t stream) {
   int* work_feats = (int*)(wh + 1);
   int* work_chunks = work_feats + F;
   if (!s->pre_zeroed) PB_CUDA(cudaMemsetAsync(wh, 0, sizeof(SaeWorkHeader), st));
-  const int grid = persistent_grid(8, F);
-  PB_DISPATCH_CHUNKS(ch, PB_LAUNCH_PDL(k_sae_grads<C_>, grid, 256, sizeof(float) * d, st, s->csc_off, s->csc_entries, s->val, s->dval, s->g, s->sae_in,
-                                       s->W_encT, s->gW_dec, s->gW_encT, s->gb_enc, s->gbdec2, s->fired, (SaeScalars*)s->scalars, F, d, s->k, wh,
-                                       work_feats, work_chunks));
-  PB_DISPATCH_CHUNKS(ch, PB_LAUNCH_PDL(k_sae_grads_long<C_>, pb_sm_count() * 4, 256, sizeof(float) * d, st, s->csc_off, s->csc_entries, s->val, s->dval,
-                                       s->g, s->sae_in, s->W_encT, s->gW_dec, s->gW_encT, s->gb_enc, s->gbdec2, s->fired, d, s->k, wh, work_chunks));
+  if (wch > 0) {
+    const int nsl = (d / 4 + SAE_SLICE_VEC - 1) / SAE_SLICE_VEC;
+    PB_LAUNCH_PDL(k_sae_grads_wide, persistent_grid(8, F * nsl), 256, sizeof(float) * d, st, s->csc_off, s->csc_entries, s->val, s->dval, s->g,
+                  s->sae_in, s->W_encT, s->gW_dec, s->gW_encT, s->gb_enc, s->gbdec2, s->fired, (SaeScalars*)s->scalars, F, d, s->k, nsl, wh,
+                  work_feats, work_chunks);
+    PB_LAUNCH_PDL(k_sae_grads_long_wide, pb_sm_count() * 4, 256, sizeof(float) * d, st, s->csc_off, s->csc_entries, s->val, s->dval, s->g,
+                  s->sae_in, s->W_encT, s->gW_dec, s->gW_encT, s->gb_enc, s->gbdec2, s->fired, d, s->k, nsl, wh, work_chunks);
+  } else {
+    const int grid = persistent_grid(8, F);
+    PB_DISPATCH_CHUNKS(ch, PB_LAUNCH_PDL(k_sae_grads<C_>, grid, 256, sizeof(float) * d, st, s->csc_off, s->csc_entries, s->val, s->dval, s->g, s->sae_in,
+                                         s->W_encT, s->gW_dec, s->gW_encT, s->gb_enc, s->gbdec2, s->fired, (SaeScalars*)s->scalars, F, d, s->k, wh,
+                                         work_feats, work_chunks));
+    PB_DISPATCH_CHUNKS(ch, PB_LAUNCH_PDL(k_sae_grads_long<C_>, pb_sm_count() * 4, 256, sizeof(float) * d, st, s->csc_off, s->csc_entries, s->val, s->dval,
+                                         s->g, s->sae_in, s->W_encT, s->gW_dec, s->gW_encT, s->gb_enc, s->gbdec2, s->fired, d, s->k, wh, work_chunks));
+  }
   if (!s->dist) {
     PB_LAUNCH_PDL(k_sae_norm_long, pb_sm_count(), 256, 0, st, s->gW_dec, s->gW_encT, s->gb_enc, (SaeScalars*)s->scalars, d, wh, work_feats);
   }
@@ -1142,7 +1675,8 @@ extern "C" int pb_sae_adam(const PbSaeStep* s, pb_stream_t stream) {
                "pb_sae_adam: missing pointers");
   PB_CHECK_ARG(s->step >= 1, "pb_sae_adam: step counter starts at 1");
   cudaStream_t st = (cudaStream_t)stream;
-  const int d = s->d, F = s->F, ch = chunks_for(d);
+  const int d = s->d, F = s->F, ch = chunks_for(d), wch = wide_chunks_for(d);
+  if (ch < 0 && wch < 0) PB_SAE_D_UNSUPPORTED();
   const AdamHyper h = adam_hyper(s->lr, s->beta1, s->beta2, s->adam_eps, s->step);
   const int grid = persistent_grid(8, F);
   PB_CHECK_ARG(!s->W_encT16 == !s->enc16_lo_max, "pb_sae_adam: W_encT16 and enc16_lo_max go together");
@@ -1150,7 +1684,7 @@ extern "C" int pb_sae_adam(const PbSaeStep* s, pb_stream_t stream) {
   __half* const W16 = (__half*)s->W_encT16;
   if (s->enc_norm_max) PB_CUDA(cudaMemsetAsync(s->enc_norm_max, 0, 2 * sizeof(float), st));
   if (s->enc16_lo_max) PB_CUDA(cudaMemsetAsync(s->enc16_lo_max, 0, sizeof(float), st));
-  if (!s->W_encT_lo && d >= 64) {      // no tf32 residual plane to maintain: the bulk-copy pipeline
+  if (!s->W_encT_lo && d >= 64 && ch > 0) {      // no tf32 residual plane to maintain, a narrow row: the bulk-copy pipeline
     const size_t stage = (size_t)8 * d * 4;
     int S = (int)((200 * 1024) / stage);
     if (S > 12) S = 12;
@@ -1168,11 +1702,18 @@ extern "C" int pb_sae_adam(const PbSaeStep* s, pb_stream_t stream) {
       return PB_OK;
     }
   }
-  PB_DISPATCH_CHUNKS(ch, (k_sae_adam_rows<C_><<<grid, 256, 0, st>>>(s->W_dec, s->W_encT, s->W_encT_lo, W16, s->enc16_lo_max, s->b_enc, s->gW_dec,
-                                                                     s->gW_encT, s->gb_enc,
-                                                                     s->m_dec, s->v_dec, s->m_enc, s->v_enc, s->m_be, s->v_be, s->fired,
-                                                                     s->since_fired, s->act_freq, (const SaeScalars*)s->scalars, h,
-                                                                     F, d, s->renorm_decoder, s->enc_norm_max)));
+  if (wch > 0) {      // wide rows: one feature per CTA (bulk copy would fit fewer than 3 ring stages)
+    PB_DISPATCH_WIDE(wch, (k_sae_adam_rows_wide<C_><<<persistent_grid(1, F), SAE_WIDE_THREADS, 0, st>>>(
+                              s->W_dec, s->W_encT, s->W_encT_lo, W16, s->enc16_lo_max, s->b_enc, s->gW_dec, s->gW_encT, s->gb_enc, s->m_dec,
+                              s->v_dec, s->m_enc, s->v_enc, s->m_be, s->v_be, s->fired, s->since_fired, s->act_freq,
+                              (const SaeScalars*)s->scalars, h, F, d, s->renorm_decoder, s->enc_norm_max)));
+  } else {
+    PB_DISPATCH_CHUNKS(ch, (k_sae_adam_rows<C_><<<grid, 256, 0, st>>>(s->W_dec, s->W_encT, s->W_encT_lo, W16, s->enc16_lo_max, s->b_enc, s->gW_dec,
+                                                                       s->gW_encT, s->gb_enc,
+                                                                       s->m_dec, s->v_dec, s->m_enc, s->v_enc, s->m_be, s->v_be, s->fired,
+                                                                       s->since_fired, s->act_freq, (const SaeScalars*)s->scalars, h,
+                                                                       F, d, s->renorm_decoder, s->enc_norm_max)));
+  }
   PB_LAUNCH_CHECK();
   k_sae_adam_vec<<<(d + 255) / 256, 256, 0, st>>>(s->b_dec, s->gb_dec, s->m_bd, s->v_bd, (const SaeScalars*)s->scalars, h, d);
   PB_LAUNCH_CHECK();
@@ -1192,10 +1733,15 @@ extern "C" int pb_adam_vec(float* p, const float* g, float* m, float* v, int32_t
 
 extern "C" int pb_unit_norm_rows(float* W, float* W_lo, int32_t F, int32_t d, pb_stream_t stream) {
   PB_CHECK_ARG(W && F >= 0 && d > 0, "pb_unit_norm_rows: bad arguments");
+  const int ch = chunks_for(d), wch = wide_chunks_for(d);
+  if (ch < 0 && wch < 0) PB_SAE_D_UNSUPPORTED();
   if (F == 0) return PB_OK;
-  const int ch = chunks_for(d);
   cudaStream_t st = (cudaStream_t)stream;
-  PB_DISPATCH_CHUNKS(ch, (k_unit_rows<C_><<<persistent_grid(8, F), 256, 0, st>>>(W, W_lo, F, d)));
+  if (wch > 0) {
+    PB_DISPATCH_WIDE(wch, (k_unit_rows_wide<C_><<<persistent_grid(1, F), SAE_WIDE_THREADS, 0, st>>>(W, W_lo, F, d)));
+  } else {
+    PB_DISPATCH_CHUNKS(ch, (k_unit_rows<C_><<<persistent_grid(8, F), 256, 0, st>>>(W, W_lo, F, d)));
+  }
   PB_LAUNCH_CHECK();
   return PB_OK;
 }

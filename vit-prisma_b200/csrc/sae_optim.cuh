@@ -72,22 +72,55 @@ __device__ __forceinline__ void dead_feature_counters(float* since_fired, float*
 }
 
 // ---------------------------------------------------------------------------------------------
-// The update of one feature by one warp (lane l holds columns 4 (i * 32 + l) .. +3 of chunk i).  The row pointers (parameters,
+// Who holds a row.  WarpRow: one warp (d <= 1536, the narrow kernels).  CtaRow: the SAE_WIDE_THREADS threads of a CTA (the wide
+// kernels, 1536 < d <= 8192); its sums go through shared memory (red: SAE_WIDE_WARPS floats) and end in a barrier, so every
+// thread of the CTA must reach each one.  Thread t() of a row holds columns 4 (i * kThreads + t()) .. +3 of chunk i.
+constexpr int SAE_WIDE_THREADS = 256;
+constexpr int SAE_WIDE_WARPS = SAE_WIDE_THREADS / 32;
+constexpr int SAE_NARROW_MAX_D = 1536;
+constexpr int SAE_WIDE_MAX_D = 8192;
+
+// sum of v over the CTA (every thread gets it, added in the same warp order)
+__device__ __forceinline__ float cta_sum(float v, float* red) {
+  v = warp_sum(v);
+  __syncthreads();                        // every thread has read the previous sum out of red
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  float s = 0.f;
+#pragma unroll
+  for (int w = 0; w < SAE_WIDE_WARPS; ++w) s += red[w];
+  return s;
+}
+
+struct WarpRow {
+  static constexpr int kThreads = 32;
+  __device__ __forceinline__ int t() const { return threadIdx.x & 31; }
+  __device__ __forceinline__ float sum(float v) const { return warp_sum(v); }
+};
+struct CtaRow {
+  float* red;
+  static constexpr int kThreads = SAE_WIDE_THREADS;
+  __device__ __forceinline__ int t() const { return threadIdx.x; }
+  __device__ __forceinline__ float sum(float v) const { return cta_sum(v, red); }
+};
+
+// ---------------------------------------------------------------------------------------------
+// The update of one feature by one row holder (a warp, or with CtaRow a CTA; below "lane" is the holder's thread index t()).  The row pointers (parameters,
 // gradients, Adam moments; global or shared memory) are read; the moments are written back in place; the updated parameter rows
 // go to out.dec(c4, w) / out.enc(c4, p, lo, p16) (lo = tf32 residual of p, p16 = fp16 copy of p, packed), which decide where they
 // are stored.  Returns this lane's partials of ||w_enc||^2, ||w_enc - trunc(w_enc)||^2 and ||w_enc - fp16(w_enc)||^2 (the fused
 // encoder's error bounds) in esq / elo / e16; a caller that stores no fp16 copy ignores e16 and the compiler drops its arithmetic.
-template <int CHUNKS, class Out>
+template <int CHUNKS, class Out, class Row = WarpRow>
 __device__ __forceinline__ void sae_adam_feature(const float* wd, const float* gd, float* md, float* vd, const float* we, const float* ge,
                                                  float* me, float* ve, float clip, const AdamHyper& h, int nvec, bool renorm,
-                                                 const Out& out, float& esq, float& elo, float& e16) {
-  const int lane = threadIdx.x & 31;
+                                                 const Out& out, float& esq, float& elo, float& e16, const Row& row = Row()) {
+  const int lane = row.t();
   // ---- decoder row: clip, remove the component parallel to the (unit-norm) row, Adam, renormalise
   float w[CHUNKS][4], gq[CHUNKS][4];
   float par = 0.f;
 #pragma unroll
   for (int i = 0; i < CHUNKS; ++i) {
-    const int c4 = i * 32 + lane;
+    const int c4 = i * Row::kThreads + lane;
     if (c4 < nvec) {
       ld4(wd + 4 * c4, w[i]);
       ld4(gd + 4 * c4, gq[i]);
@@ -97,11 +130,11 @@ __device__ __forceinline__ void sae_adam_feature(const float* wd, const float* g
       w[i][0] = w[i][1] = w[i][2] = w[i][3] = gq[i][0] = gq[i][1] = gq[i][2] = gq[i][3] = 0.f;
     }
   }
-  par = warp_sum(par);
+  par = row.sum(par);
   float nsq = 0.f;
 #pragma unroll
   for (int i = 0; i < CHUNKS; ++i) {
-    const int c4 = i * 32 + lane;
+    const int c4 = i * Row::kThreads + lane;
     if (c4 < nvec) {
       float mm[4], vv[4];
       ld4(md + 4 * c4, mm);
@@ -115,10 +148,10 @@ __device__ __forceinline__ void sae_adam_feature(const float* wd, const float* g
       st4(vd + 4 * c4, vv);
     }
   }
-  const float inv_nrm = 1.f / sqrtf(warp_sum(nsq));
+  const float inv_nrm = 1.f / sqrtf(row.sum(nsq));
 #pragma unroll
   for (int i = 0; i < CHUNKS; ++i) {
-    const int c4 = i * 32 + lane;
+    const int c4 = i * Row::kThreads + lane;
     if (c4 < nvec) {
       if (renorm) {
 #pragma unroll
@@ -133,7 +166,7 @@ __device__ __forceinline__ void sae_adam_feature(const float* wd, const float* g
   e16 = 0.f;
 #pragma unroll
   for (int i = 0; i < CHUNKS; ++i) {
-    const int c4 = i * 32 + lane;
+    const int c4 = i * Row::kThreads + lane;
     if (c4 < nvec) {
       float p[4], gr[4], mm[4], vv[4], lo[4];
       ld4(we + 4 * c4, p);
@@ -156,7 +189,8 @@ __device__ __forceinline__ void sae_adam_feature(const float* wd, const float* g
 }
 
 // ---------------------------------------------------------------------------------------------
-// host side: row kernels are instantiated per CHUNKS = ceil(d / 128) rounded up to a built width (d <= 1536, d % 4 == 0)
+// host side: the narrow row kernels are instantiated per CHUNKS = ceil(d / 128) rounded up to a built width (d <= 1536,
+// d % 4 == 0), the wide ones per CHUNKS = ceil(d / 1024) rounded up to a built width (1536 < d <= 8192, d % 4 == 0)
 static inline int chunks_for(int d) {
   if (d % 4 != 0) return -1;
   const int nvec = d / 4;
@@ -168,6 +202,19 @@ static inline int chunks_for(int d) {
   if (nvec <= 384) return 12;
   return -1;
 }
+static inline int wide_chunks_for(int d) {
+  if (d % 4 != 0 || d <= SAE_NARROW_MAX_D || d > SAE_WIDE_MAX_D) return -1;
+  const int nvec = d / 4;
+  if (nvec <= 2 * SAE_WIDE_THREADS) return 2;
+  if (nvec <= 4 * SAE_WIDE_THREADS) return 4;
+  if (nvec <= 6 * SAE_WIDE_THREADS) return 6;
+  return 8;
+}
+#define PB_SAE_D_UNSUPPORTED()                                                                                      \
+  do {                                                                                                              \
+    pb_set_error("sae: d_in=%d unsupported (needs d %% 4 == 0 and d <= 8192)", d);                                  \
+    return PB_EUNSUPPORTED;                                                                                         \
+  } while (0)
 #define PB_DISPATCH_CHUNKS(CH, ...)                                                    \
   switch (CH) {                                                                        \
     case 1: { constexpr int C_ = 1; __VA_ARGS__; } break;                              \
@@ -176,5 +223,13 @@ static inline int chunks_for(int d) {
     case 6: { constexpr int C_ = 6; __VA_ARGS__; } break;                              \
     case 8: { constexpr int C_ = 8; __VA_ARGS__; } break;                              \
     case 12: { constexpr int C_ = 12; __VA_ARGS__; } break;                            \
-    default: pb_set_error("sae: d_in=%d unsupported (needs d %% 4 == 0 and d <= 1536)", d); return PB_EUNSUPPORTED; \
+    default: PB_SAE_D_UNSUPPORTED();                                                   \
+  }
+#define PB_DISPATCH_WIDE(CH, ...)                                                      \
+  switch (CH) {                                                                        \
+    case 2: { constexpr int C_ = 2; __VA_ARGS__; } break;                              \
+    case 4: { constexpr int C_ = 4; __VA_ARGS__; } break;                              \
+    case 6: { constexpr int C_ = 6; __VA_ARGS__; } break;                              \
+    case 8: { constexpr int C_ = 8; __VA_ARGS__; } break;                              \
+    default: PB_SAE_D_UNSUPPORTED();                                                   \
   }

@@ -17,10 +17,11 @@ import torch
 
 from . import _lib as L
 from .ops import _stream
-from .sae_engine import PbSaeEncode, PbSaeStep, SaeStepEngine, ops_cast_f32
+from .sae_engine import MAX_D_IN, NARROW_MAX_D_IN, PbSaeEncode, PbSaeStep, SaeStepEngine, ops_cast_f32
 
 vp, i32, i64, f32, u32, u64 = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_uint32, C.c_uint64
 MAX_RANKS = 8
+DP_MAX_D_IN = NARROW_MAX_D_IN      # widest d_in of the peer-memory optimizer (k_p2p_adam_allgather's one-warp rows)
 _TABLES = ("gW_dec", "gW_encT", "gb_enc", "gb_dec", "fired", "xsum", "W_dec", "W_encT", "W_encT_lo", "b_enc", "norm_parts", "flags")
 
 
@@ -231,8 +232,11 @@ class SaeDPEngine(SaeStepEngine):
     is_data_parallel = True
 
     def __init__(self, group: P2PGroup, W_encT: torch.Tensor, W_dec: torch.Tensor, b_enc: torch.Tensor, b_dec: torch.Tensor, k: int, **kw):
-        self.group = group
         F, d = W_dec.shape
+        if d > DP_MAX_D_IN:          # k_p2p_adam_allgather holds a row in one warp; refused before any peer allocation
+            raise L.PrismaB200Error(f"SaeDPEngine: d_in={d} unsupported by the data-parallel optimizer (d_in <= {DP_MAX_D_IN}; "
+                                    f"the single-GPU engine takes d_in up to {MAX_D_IN})")
+        self.group = group
         shard_bounds(F, group.rank, group.world)
         g = group
         # parameters + gradient matrices: one NVSwitch multicast pool when the fabric offers it (multimem.ld_reduce / multimem.st in

@@ -78,6 +78,8 @@ L.register_signatures({
 NORM_MODE = {"none": 0, None: 0, "layer_norm": 1, "constant_norm_rescale": 2}
 SCALAR_NAMES = ("loss_sum", "gnorm_sq", "clip_coef", "mse", "l0", "pos_count", "grad_norm", "reserved")
 TOPK_SEG = 256 * 96
+NARROW_MAX_D_IN = 1536     # widest d_in of the one-warp-per-row step kernels; past it the wide (one CTA per row) kernels run
+MAX_D_IN = 8192            # widest d_in of every SAE step kernel (and of the fused encoder)
 
 
 def unit_norm_rows_(w: torch.Tensor, w_lo: Optional[torch.Tensor] = None) -> None:
@@ -148,6 +150,8 @@ class SaeStepEngine:
             if t.dtype != torch.float32 or not t.is_contiguous():
                 raise L.PrismaB200Error("SaeStepEngine: parameters must be contiguous fp32 CUDA tensors")
         self.F, self.d = W_dec.shape
+        if self.d > MAX_D_IN:          # refused before any allocation or launch (d % 4 != 0 is refused by refresh_lo's pb_rownorm_max)
+            raise L.PrismaB200Error(f"sae: d_in={self.d} unsupported (needs d % 4 == 0 and d <= {MAX_D_IN})")
         assert W_encT.shape == (self.F, self.d) and b_enc.shape == (self.F,) and b_dec.shape == (self.d,)
         self.k = int(k)
         self.W_encT, self.W_dec, self.b_enc, self.b_dec = W_encT, W_dec, b_enc, b_dec
@@ -353,7 +357,10 @@ class SaeStepEngine:
     def _optimizer_stages(self, s: PbSaeStep, x: torch.Tensor, lr: float, since_fired, act_freq):
         """(name, callable, info) of the stages after backward; the data-parallel engine replaces them with its peer-memory phases."""
         lib, st = L.get_lib(), _stream()
-        kernel = "k_sae_adam_rows" if self.W_encT_lo is not None or self.d < 64 else "k_sae_adam_bulk"   # pb_sae_adam's choice
+        if self.d > NARROW_MAX_D_IN:                                          # pb_sae_adam's choice
+            kernel = "k_sae_adam_rows_wide"
+        else:
+            kernel = "k_sae_adam_rows" if self.W_encT_lo is not None or self.d < 64 else "k_sae_adam_bulk"
         f16_copy = 2 * self.d * self.F if self.W_encT16 is not None else 0      # + the fp16 copy of W_enc
         return [("adam (clip + decoder-parallel-gradient removal + Adam + row renorm)", lambda: L.check(lib.pb_sae_adam(C.byref(s), st)),
                  dict(bytes=60 * self.d * self.F + f16_copy, ncu=kernel))]
@@ -403,7 +410,7 @@ class SaeStepEngine:
         timed("decode (sparse decode + loss + d_hidden)", lambda: L.check(lib.pb_sae_decode(C.byref(s), st)),
               bytes=(12 * rows * self.d + 8 * rows * self.k), ncu=r"k_sae_decode")
         timed("backward (csc build + per-feature gradients + norm)", lambda: (self.scalars.zero_(), L.check(lib.pb_sae_backward(C.byref(s), st))),
-              bytes=8 * self.d * self.F, ncu=r"k_sae_grads<")
+              bytes=8 * self.d * self.F, ncu=r"k_sae_grads<" if self.d <= NARROW_MAX_D_IN else r"k_sae_grads_wide")
         for name, fn, info in self._optimizer_stages(s, x, float(lr), since_fired, act_freq):
             timed(name, fn, **info)
         return out
